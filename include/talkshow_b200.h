@@ -84,6 +84,13 @@ int ts_pixelcnn_generate(ts_engine* e, const float* aud, const int64_t* label, c
 /* GatedPixelCNN.forward (teacher forced), :130-150, for rows [0,T): logits_out [B,2048,T,2]. */
 int ts_pixelcnn_logits(ts_engine* e, const float* aud, const int64_t* label, const int64_t* codes,
                        float* logits_out, int B, int T, void* stream);
+/* Teacher-forced GatedPixelCNN.forward (:130-150) over all rows at once + per-position cross-entropy
+ * (nets/smplx_body_pixel.py:207-216 without the update).  aud [B,256,T], label [B], codes [B,T,2] int64 ->
+ * nll_out [B,T,2] = -log softmax(logits)[code]; logits_out (may be NULL) [B,2048,T,2].  Any B, any T >= 1.
+ * No serial dependency: a fixed number of launches (large GEMMs over all B*T*2 positions) whatever T is.
+ * Dense layers run on the kernel ts_set_tensor_cores selects. */
+int ts_pixelcnn_score(ts_engine* e, const float* aud, const int64_t* label, const int64_t* codes,
+                      float* nll_out, float* logits_out, int B, int T, void* stream);
 
 /* VQVAE.decode(latents=...), nets/spg/vqvae_1d.py:201-208: idx [B,T] int64 -> out [B,C,4T]
  * (C = ts_vq_dim(which): 39 body / 90 hand, 78 / 180 for 6-D).  The indices are device data and are NOT range-checked (the

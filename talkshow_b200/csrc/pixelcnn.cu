@@ -1314,6 +1314,7 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
 void pixel_destroy(ts_engine* e) {
   if (!e->pix) return;
   delete (Plan3*)e->pix->p3;
+  tf_free(e->pix->tf);
   delete e->pix;
   e->pix = nullptr;
 }
@@ -1349,6 +1350,7 @@ extern "C" int ts_load_pixelcnn(ts_engine* e, const ts_tensor* tensors, int n) {
   Plan3* Q = (P->has_v1 && e->pixel_ctas > 0) ? nullptr : build_plan3(e, ck, L, D, ncls);
   P->p3 = Q;
   if (!P->has_v1) { P->nstages = Q->nstages; P->ncta = C3_CL; }
+  P->tf = tf_build(e, ck, L, D, ncls);
   pixel_destroy(e);
   e->pix = P.release();
   scope.commit();

@@ -63,6 +63,7 @@ struct PixelPlan {
   unsigned* d_barrier = nullptr;
   Layer emb_aud, fuse_v_a, fuse_h_a;  // audio terms (precomputed per call for all rows)
   void* p3 = nullptr;          // Plan3 of the cluster-resident executor (pixelcnn3.inc)
+  void* tf = nullptr;          // TfPlan of the time-parallel teacher-forced scorer (pixelcnn_tf.cu)
   unsigned long long* d_trace = nullptr;  // stage trace buffer (ts_pixelcnn_trace)
   int trace_row = -1;
   bool timing = false, pending = false;
@@ -77,6 +78,9 @@ void pixelcnn_generate_act(ts_engine* e, const Act3& aud, const int64_t* label, 
 // idx [B,T,2] -> idx_c [2][B][T]; optionally copies idx to codes_out
 void split_codes(ts_engine* e, const int64_t* idx, int64_t* idx_c, int B, int T, int64_t* codes_out, cudaStream_t s);
 void pixel_destroy(ts_engine* e);
+// weights of ts_pixelcnn_score packed for its GEMMs (pixelcnn_tf.cu); nullptr on a host-only engine
+void* tf_build(ts_engine* e, const Ckpt& ck, int L, int D, int ncls);
+void tf_free(void* p);
 void face_destroy(ts_engine* e);
 void mfcc_destroy(ts_engine* e);
 void smplx_destroy(ts_engine* e);

@@ -204,6 +204,24 @@ class Engine:
                                               B, T, self._s()), "ts_pixelcnn_logits")
         return out
 
+    def pixelcnn_score(self, aud, label, codes, want_logits=False):
+        """Teacher-forced GatedPixelCNN.forward over all rows at once + per-position cross-entropy: aud [B,256,T],
+        label [B], codes [B,T,2] -> nll [B,T,2] = -log softmax(logits)[code] (+ logits [B,2048,T,2]).  Any batch size."""
+        aud = self._dev(aud, torch.float32)
+        label = self._dev(label, torch.int64).reshape(-1)
+        codes = self._dev(codes, torch.int64)
+        B, _, T = aud.shape
+        if label.numel() == 1 and B > 1:
+            label = label.expand(B).contiguous()
+        if aud.shape[1] != 256 or tuple(codes.shape) != (B, T, 2) or label.numel() != B:
+            raise ValueError("pixelcnn_score: aud %s, label %s, codes %s (expected [B,256,T], [B], [B,T,2])"
+                             % (tuple(aud.shape), tuple(label.shape), tuple(codes.shape)))
+        nll = torch.empty(B, T, 2, device=self.device)
+        logits = torch.empty(B, 2048, T, 2, device=self.device) if want_logits else None
+        self._check(self.L.ts_pixelcnn_score(self.h, _lib.ptr(aud), _lib.ptr(label), _lib.ptr(codes), _lib.ptr(nll),
+                                             _lib.ptr(logits), B, T, self._s()), "ts_pixelcnn_score")
+        return (nll, logits) if want_logits else nll
+
     def vq_dim(self, which):
         """pose channels of the loaded VQ-VAE: 39 / 90 (axis-angle), 78 / 180 (convert_to_6d)."""
         c = int(self.L.ts_vq_dim(self.h, which))

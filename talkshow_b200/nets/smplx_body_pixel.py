@@ -77,6 +77,30 @@ class TrainWrapper:
         return {"generator": loaded["generator"], "generator_optim": None, "audioencoder": loaded["audioencoder"],
                 "audioencoder_optim": None, "discriminator": None, "discriminator_optim": None}
 
+    # -- evaluation ------------------------------------------------------------------------------
+    def evaluate(self, bat):
+        """The forward half of the reference's training step __call__(bat) (:183-216) in validation mode (BatchNorm
+        running statistics, dropout off): ground-truth poses -> VQ codes, audio features -> AudioEncoder, one
+        teacher-forced prior forward over all rows, cross-entropy against the codes.  bat: 'aud_feat' [B,64,M],
+        'poses' [B,C,F] (165 axis-angle channels, or the 6-D layout), 'speaker' [B] (id = speaker - 20).
+        Returns (None, {'ce_loss': float}); the per-position NLL [B,T,2] is kept as self.last_nll."""
+        aud = bat["aud_feat"].to(torch.float32)
+        poses = bat["poses"].to(torch.float32)
+        label = (torch.as_tensor(bat["speaker"]) - 20).reshape(-1).to(torch.int64)
+        gt = poses[:, self.c_index, :].permute(0, 2, 1)                       # [B,F,C]
+        nb = self.each_dim[1]
+        body = self.engine.vq_encode(0, gt[..., :nb].contiguous())
+        hand = self.engine.vq_encode(1, gt[..., nb:].contiguous())
+        latents = torch.stack([body, hand], -1)                               # [B,T,2]
+        audio = self.engine.audio_encode(aud)                                 # [B,256,Ta]
+        if audio.shape[2] != latents.shape[1]:
+            # the reference fails in the prior's concatenation of code and audio rows (gated_pixelcnn_v2.py:143)
+            raise ValueError("evaluate: %d audio rows (%d feature frames) vs %d code rows (%d pose frames)"
+                             % (audio.shape[2], aud.shape[2], latents.shape[1], poses.shape[2]))
+        nll = self.engine.pixelcnn_score(audio, label, latents)
+        self.last_nll = nll
+        return None, {"ce_loss": float(nll.double().mean())}
+
     # -- inference -------------------------------------------------------------------------------
     def _noise(self, T, B):
         return draw_sampler_noise(T, B, self.noise_device, per_step=self.noise_per_step)
