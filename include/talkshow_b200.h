@@ -101,9 +101,16 @@ int ts_vq_encode(ts_engine* e, int which, const float* poses, int64_t* idx, floa
                  void* stream);
 
 /* s2g_face.Generator.forward, nets/spg/s2g_face.py:196-224: wave [B,N] (16 kHz), id [B,4] float
- * one-hot (zeros = "no id", nets/smplx_face.py:205-206) -> out [B,frame,103]. */
+ * one-hot (zeros = "no id", nets/smplx_face.py:205-206) -> out [B,frame,ts_face_dim(e)].
+ * The net's geometry is read from the checkpoint by ts_load_face: with 'audio_middle.id_mlp.*' it is the identity net
+ * (3-D jaw, 103 columns); without, the identity-free net of convert_to_6d configs (AudioEncoder identity=False, 6-D jaw,
+ * 106 columns), which ignores `id` (it may be NULL). */
 int ts_face_forward(ts_engine* e, const float* wave, const float* id, float* out, int B, int N, int frame,
                     void* stream);
+
+/* output columns of the loaded face net: 103 (jaw 3 + expression 100) or 106 (6-D jaw 6 + expression 100);
+ * 0 when no face is loaded. */
+int ts_face_dim(ts_engine* e);
 
 /* pose channels of the loaded VQ-VAE `which` (in_dim of nets/smplx_body_pixel.py:54-57: 39 / 90 axis-angle,
  * 78 / 180 with convert_to_6d); 0 when not loaded. */
@@ -125,6 +132,12 @@ int ts_mfcc_frames(int N, int sr);
  * body [B,Fb,129] -> out [B,Ff,265]; body is padded with its last frame / truncated to Ff. */
 int ts_assemble_pose(ts_engine* e, const float* face, const float* body, float* out, int B, int Ff, int Fb,
                      int stand, void* stream);
+
+/* The convert_to_6d form of ts_assemble_pose: face [B,Ff,106] (6-D jaw | expression), body [B,Fb,258] (43 joints x 6-D)
+ * -> out [B,Ff,265].  Each jaw / body joint is converted to axis-angle inside the assembly kernel with the arithmetic of
+ * ts_rot6d_to_axis_angle, so the result equals ts_rot6d_to_axis_angle followed by ts_assemble_pose bit for bit. */
+int ts_assemble_pose6d(ts_engine* e, const float* face, const float* body, float* out, int B, int Ff, int Fb,
+                       int stand, void* stream);
 
 /* scripts/demo.py:185-188,216-219 (convert_to_6d configs): matrix_to_axis_angle(rotation_6d_to_matrix(x)),
  * data_utils/rotation_conversion.py:512-533,433-447.  d6 [n,6] -> aa [n,3] (device pointers). */

@@ -110,10 +110,53 @@ __constant__ float c_lower_pose[33] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 3.074
     -0.1603458970785141f, 1.1654603481292725f, 0.0f, 0.0f, 1.2521806955337524f, 0.041598282754421234f,
     -0.06312154978513718f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
 
+// ---- 6-D rotation -> axis-angle: matrix_to_axis_angle(rotation_6d_to_matrix(x)) ----------------------
+// (data_utils/rotation_conversion.py:512-533 Gram-Schmidt, :98-118 matrix_to_quaternion, :481-507
+// quaternion_to_axis_angle; applied by scripts/demo.py:185-188,216-219 when convert_to_6d is set).
+// One definition for rot6d_to_aa_kernel and the fused 6-D assembly, so the two give the same bits.
+__device__ __forceinline__ void rot6d_to_aa(const float* __restrict__ p, float& ax, float& ay, float& az) {
+  const float a1x = p[0], a1y = p[1], a1z = p[2], a2x = p[3], a2y = p[4], a2z = p[5];
+  float n1 = fmaxf(sqrtf(a1x * a1x + a1y * a1y + a1z * a1z), 1e-12f);           // F.normalize eps
+  const float b1x = a1x / n1, b1y = a1y / n1, b1z = a1z / n1;
+  const float d = b1x * a2x + b1y * a2y + b1z * a2z;
+  float b2x = a2x - d * b1x, b2y = a2y - d * b1y, b2z = a2z - d * b1z;
+  float n2 = fmaxf(sqrtf(b2x * b2x + b2y * b2y + b2z * b2z), 1e-12f);
+  b2x /= n2; b2y /= n2; b2z /= n2;
+  const float b3x = b1y * b2z - b1z * b2y, b3y = b1z * b2x - b1x * b2z, b3z = b1x * b2y - b1y * b2x;
+  // rows of the matrix are b1, b2, b3
+  const float m00 = b1x, m11 = b2y, m22 = b3z;
+  auto sqp = [](float v) { return v > 0.f ? sqrtf(v) : 0.f; };                     // _sqrt_positive_part
+  const float q0 = 0.5f * sqp(1.f + m00 + m11 + m22);
+  float q1 = 0.5f * sqp(1.f + m00 - m11 - m22);
+  float q2 = 0.5f * sqp(1.f - m00 + m11 - m22);
+  float q3 = 0.5f * sqp(1.f - m00 - m11 + m22);
+  if (b3y - b2z < 0.f) q1 = -q1;        // _copysign(x, m21 - m12)
+  if (b1z - b3x < 0.f) q2 = -q2;        // _copysign(y, m02 - m20)
+  if (b2x - b1y < 0.f) q3 = -q3;        // _copysign(z, m10 - m01)
+  const float nv = sqrtf(q1 * q1 + q2 * q2 + q3 * q3);
+  const float half = atan2f(nv, q0), ang = 2.f * half;
+  const float sh = fabsf(ang) < 1e-6f ? 0.5f - (ang * ang) / 48.f : sinf(half) / ang;
+  ax = q1 / sh;
+  ay = q2 / sh;
+  az = q3 / sh;
+}
+
+// component c (0..2) of the axis-angle of the 6-D rotation at p
+__device__ __forceinline__ float rot6d_aa_component(const float* __restrict__ p, int c) {
+  float x, y, z;
+  rot6d_to_aa(p, x, y, z);
+  return c == 0 ? x : (c == 1 ? y : z);
+}
+
 // out column -> source: pred = cat[jaw(3), body(129), expr(100)] (232), part2full inserts lower-pose
 // blocks: [pred 0:3 | lp 0:15 | pred 3:6 | lp 15:21 | pred 6:9 | lp 21:27 | pred 9:12 | lp 27:33 | pred 12:232]
+// SIX = false: face [B,Ff,103] = jaw(3) | expr(100), body [B,Fb,129] axis-angle.
+// SIX = true:  face [B,Ff,106] = jaw(6-D) | expr(100), body [B,Fb,258] = 43 joints x 6-D; each needed joint is converted
+//              to axis-angle on the fly (demo.py:185-188,216-219 followed by the same assembly).
+template <bool SIX>
 __global__ void assemble_kernel(const float* __restrict__ face, const float* __restrict__ body, float* __restrict__ out,
                                 int B, int Ff, int Fb, int stand) {
+  constexpr int FD = SIX ? 106 : 103, BD = SIX ? 258 : 129, JW = SIX ? 6 : 3;
   long n = (long)B * Ff * 265;
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
     int c = i % 265;
@@ -133,61 +176,48 @@ __global__ void assemble_kernel(const float* __restrict__ face, const float* __r
     if (lp >= 0) {
       v = stand ? ((lp >= 6 && lp < 9) ? c_lower_pose[lp] : 0.f) : c_lower_pose[lp];
     } else if (pc < 3) {
-      v = face[((long)b * Ff + f) * 103 + pc];
+      const float* fr = face + ((long)b * Ff + f) * FD;
+      v = SIX ? rot6d_aa_component(fr, pc) : fr[pc];
     } else if (pc < 132) {
       int fb = f < Fb ? f : Fb - 1;
-      v = body[((long)b * Fb + fb) * 129 + (pc - 3)];
+      const float* br = body + ((long)b * Fb + fb) * BD;
+      v = SIX ? rot6d_aa_component(br + (pc - 3) / 3 * 6, (pc - 3) % 3) : br[pc - 3];
     } else {
-      v = face[((long)b * Ff + f) * 103 + 3 + (pc - 132)];
+      v = face[((long)b * Ff + f) * FD + JW + (pc - 132)];
     }
     out[i] = v;
   }
 }
 
+static void launch_assemble(ts_engine* e, bool six, const float* face, const float* body, float* out, int B, int Ff, int Fb,
+                            int stand, void* stream) {
+  ts::require_device(e);
+  if (B <= 0 || Ff <= 0 || Fb <= 0) fail(TS_ERR_INVALID, "%s: B=%d Ff=%d Fb=%d", six ? "ts_assemble_pose6d" : "ts_assemble_pose", B, Ff, Fb);
+  long n = (long)B * Ff * 265;
+  int blocks = (int)std::min<long>((n + 255) / 256, (long)e->sm_count * 8);
+  if (six) assemble_kernel<true><<<blocks, 256, 0, (cudaStream_t)stream>>>(face, body, out, B, Ff, Fb, stand);
+  else assemble_kernel<false><<<blocks, 256, 0, (cudaStream_t)stream>>>(face, body, out, B, Ff, Fb, stand);
+  e->launches++;
+  TS_CUDA(cudaGetLastError());
+}
+
 extern "C" int ts_assemble_pose(ts_engine* e, const float* face, const float* body, float* out, int B, int Ff, int Fb,
                                 int stand, void* stream) {
   TS_API_BEGIN(e)
-  ts::require_device(e);
-  if (B <= 0 || Ff <= 0 || Fb <= 0) fail(TS_ERR_INVALID, "ts_assemble_pose: B=%d Ff=%d Fb=%d", B, Ff, Fb);
-  long n = (long)B * Ff * 265;
-  int blocks = (int)std::min<long>((n + 255) / 256, (long)e->sm_count * 8);
-  assemble_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(face, body, out, B, Ff, Fb, stand);
-  e->launches++;
-  TS_CUDA(cudaGetLastError());
+  launch_assemble(e, false, face, body, out, B, Ff, Fb, stand, stream);
   TS_API_END(e)
 }
 
-// ---- 6-D rotation -> axis-angle: matrix_to_axis_angle(rotation_6d_to_matrix(x)) ----------------------
-// (data_utils/rotation_conversion.py:512-533 Gram-Schmidt, :98-118 matrix_to_quaternion, :481-507
-// quaternion_to_axis_angle; applied by scripts/demo.py:185-188,216-219 when convert_to_6d is set)
+extern "C" int ts_assemble_pose6d(ts_engine* e, const float* face, const float* body, float* out, int B, int Ff, int Fb,
+                                  int stand, void* stream) {
+  TS_API_BEGIN(e)
+  launch_assemble(e, true, face, body, out, B, Ff, Fb, stand, stream);
+  TS_API_END(e)
+}
+
 __global__ void rot6d_to_aa_kernel(const float* __restrict__ d6, float* __restrict__ aa, long n) {
-  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
-    const float* p = d6 + i * 6;
-    const float a1x = p[0], a1y = p[1], a1z = p[2], a2x = p[3], a2y = p[4], a2z = p[5];
-    float n1 = fmaxf(sqrtf(a1x * a1x + a1y * a1y + a1z * a1z), 1e-12f);           // F.normalize eps
-    const float b1x = a1x / n1, b1y = a1y / n1, b1z = a1z / n1;
-    const float d = b1x * a2x + b1y * a2y + b1z * a2z;
-    float b2x = a2x - d * b1x, b2y = a2y - d * b1y, b2z = a2z - d * b1z;
-    float n2 = fmaxf(sqrtf(b2x * b2x + b2y * b2y + b2z * b2z), 1e-12f);
-    b2x /= n2; b2y /= n2; b2z /= n2;
-    const float b3x = b1y * b2z - b1z * b2y, b3y = b1z * b2x - b1x * b2z, b3z = b1x * b2y - b1y * b2x;
-    // rows of the matrix are b1, b2, b3
-    const float m00 = b1x, m11 = b2y, m22 = b3z;
-    auto sqp = [](float v) { return v > 0.f ? sqrtf(v) : 0.f; };                     // _sqrt_positive_part
-    const float q0 = 0.5f * sqp(1.f + m00 + m11 + m22);
-    float q1 = 0.5f * sqp(1.f + m00 - m11 - m22);
-    float q2 = 0.5f * sqp(1.f - m00 + m11 - m22);
-    float q3 = 0.5f * sqp(1.f - m00 - m11 + m22);
-    if (b3y - b2z < 0.f) q1 = -q1;        // _copysign(x, m21 - m12)
-    if (b1z - b3x < 0.f) q2 = -q2;        // _copysign(y, m02 - m20)
-    if (b2x - b1y < 0.f) q3 = -q3;        // _copysign(z, m10 - m01)
-    const float nv = sqrtf(q1 * q1 + q2 * q2 + q3 * q3);
-    const float half = atan2f(nv, q0), ang = 2.f * half;
-    const float sh = fabsf(ang) < 1e-6f ? 0.5f - (ang * ang) / 48.f : sinf(half) / ang;
-    aa[i * 3 + 0] = q1 / sh;
-    aa[i * 3 + 1] = q2 / sh;
-    aa[i * 3 + 2] = q3 / sh;
-  }
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x)
+    rot6d_to_aa(d6 + i * 6, aa[i * 3 + 0], aa[i * 3 + 1], aa[i * 3 + 2]);
 }
 
 extern "C" int ts_rot6d_to_axis_angle(ts_engine* e, const float* d6, float* aa, int64_t n, void* stream) {

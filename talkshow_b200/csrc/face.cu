@@ -31,6 +31,9 @@ struct FaceNet {
   float *enc_ln_g = nullptr, *enc_ln_b = nullptr;
   std::vector<EncLayer> layers;
   Layer feat_map;
+  // identity net (audio_middle.id_mlp present): first_net layer 0 takes [feature 256 | id 64] and has a residual conv.
+  // identity-free net (the convert_to_6d face, identity=False): layer 0 takes the 256 features, residual = input.
+  bool identity = true;
   float *id_w = nullptr, *id_b = nullptr;  // [64][ncls], [64]
   int ncls = 4;
   Layer fn_conv[3], fn_res0;
@@ -1308,27 +1311,35 @@ static void face_run(ts_engine* e, const float* wave, const float* idv, float* o
     linear(e, L.ff2, ff, t1, ACT_NONE, &hcur, s);                        // h + ffn(h)
     ln_pre(e, t1, nullptr, L.ln2_g, L.ln2_b, hcur, nullptr, ACT_NONE, s);
   }
-  // ---- audio_feature_map + id_mlp concat -> first_net -------------------------------------------------
+  // ---- audio_feature_map (+ id_mlp concat on an identity net) -> first_net ------------------------------
   const bool tcf = tc && e->tc_f16;                       // first_net / decoder convs on the tensor-core kernel too (fp16 planes)
-  Act3 cat = new_act(e, B, frame, 320, 1, s, tcf);
+  Act3 cat = new_act(e, B, frame, F.identity ? 320 : 256, 1, s, tcf);
   linear(e, F.feat_map, hcur, cat, ACT_NONE, nullptr, s, 0);
-  if (!e->ws.sizing) {
+  if (F.identity && !e->ws.sizing) {
     id_cols_kernel<<<dim3(cdiv(frame * 64, 256), B), 256, 0, s>>>(idv, F.id_w, F.id_b, F.ncls, cat, 256);
     e->launches++;
     TS_CUDA(cudaGetLastError());
   }
-  Act3 c0 = new_act(e, B, frame, 256, 0, s), r0 = new_act(e, B, frame, 256, 0, s);
-  conv_auto(e, F.fn_conv[0], cat, 3, 1, 1, c0, frame, ACT_NONE, nullptr, s);
-  conv_auto(e, F.fn_res0, cat, 3, 1, 1, r0, frame, ACT_NONE, nullptr, s);
-  Act3 f = new_act(e, B, frame, 256, 1, s, tcf);
-  ln_pre(e, c0, nullptr, F.fn_g[0], F.fn_b[0], f, &r0, ACT_RELU, s);       // relu(LN(conv(x)) + conv_res(x))
+  Act3 c0 = new_act(e, B, frame, 256, 0, s);
+  Act3 f;
+  if (F.identity) {
+    Act3 r0 = new_act(e, B, frame, 256, 0, s);
+    conv_auto(e, F.fn_conv[0], cat, 3, 1, 1, c0, frame, ACT_NONE, nullptr, s);
+    conv_auto(e, F.fn_res0, cat, 3, 1, 1, r0, frame, ACT_NONE, nullptr, s);
+    f = new_act(e, B, frame, 256, 1, s, tcf);
+    ln_pre(e, c0, nullptr, F.fn_g[0], F.fn_b[0], f, &r0, ACT_RELU, s);     // relu(LN(conv(x)) + conv_res(x))
+  } else {
+    conv_auto(e, F.fn_conv[0], cat, 3, 1, 1, c0, frame, ACT_NONE, nullptr, s);
+    f = new_act(e, B, frame, 256, 1, s, tcf);
+    ln_pre(e, c0, nullptr, F.fn_g[0], F.fn_b[0], f, &cat, ACT_RELU, s);    // relu(LN(conv(x)) + x): residual is nn.Identity
+  }
   for (int i = 1; i < 3; ++i) {
     conv_auto(e, F.fn_conv[i], f, 3, 1, 1, c0, frame, ACT_NONE, nullptr, s);
     Act3 g = new_act(e, B, frame, 256, 1, s, tcf);
     ln_pre(e, c0, nullptr, F.fn_g[i], F.fn_b[i], g, &f, ACT_RELU, s);      // relu(LN(conv(x)) + x)
     f = g;
   }
-  // ---- two decoder branches -> [B, frame, 103] --------------------------------------------------------
+  // ---- two decoder branches -> [B, frame, jaw_dim + exp_dim] (103, or 106 with a 6-D jaw) ---------------
   Act3 yout;
   yout.p = out; yout.B = B; yout.T = frame; yout.C = F.jaw_dim + F.exp_dim; yout.pad = 0;
   for (int br = 0; br < 2; ++br) {
@@ -1399,14 +1410,21 @@ extern "C" int ts_load_face(ts_engine* e, const ts_tensor* tensors, int n) {
   }
   if (F->layers.empty()) fail(TS_ERR_MISSING, "face: no transformer layers in checkpoint");
   F->feat_map = pack_linear(e, ck.f32("audio_feature_map.weight", {256, 768}), ck.f32("audio_feature_map.bias", {256}), 256, 768);
-  const ts_tensor* idw = ck.get("audio_middle.id_mlp.weight");
-  F->ncls = (int)idw->shape[1];
-  F->id_w = up(e, ck.f32("audio_middle.id_mlp.weight", {64, F->ncls, 1}), (size_t)64 * F->ncls);
-  F->id_b = up(e, ck.f32("audio_middle.id_mlp.bias", {64}), 64);
+  // the geometry follows the tensors: id_mlp present -> identity net, absent -> identity-free (AudioEncoder identity=False)
   const std::string fn = "audio_middle.first_net.conv_layers.";
-  F->fn_res0 = pack_ckc(e, ck.f32(fn + "0.residual_layer.0.weight", {256, 320, 3}), ck.f32(fn + "0.residual_layer.0.bias", {256}), 256, 320, 3);
+  F->identity = ck.has("audio_middle.id_mlp.weight");
+  if (F->identity) {
+    const ts_tensor* idw = ck.get("audio_middle.id_mlp.weight");
+    F->ncls = (int)idw->shape[1];
+    F->id_w = up(e, ck.f32("audio_middle.id_mlp.weight", {64, F->ncls, 1}), (size_t)64 * F->ncls);
+    F->id_b = up(e, ck.f32("audio_middle.id_mlp.bias", {64}), 64);
+    F->fn_res0 = pack_ckc(e, ck.f32(fn + "0.residual_layer.0.weight", {256, 320, 3}), ck.f32(fn + "0.residual_layer.0.bias", {256}), 256, 320, 3);
+  } else if (ck.has(fn + "0.residual_layer.0.weight")) {
+    fail(TS_ERR_MISSING, "face: checkpoint tensor '%s0.residual_layer.0.weight' present but 'audio_middle.id_mlp.weight' missing "
+         "(an identity-free net has no residual conv in layer 0)", fn.c_str());
+  }
   for (int i = 0; i < 3; ++i) {
-    int cin = i == 0 ? 320 : 256;
+    int cin = (i == 0 && F->identity) ? 320 : 256;
     const std::string p = fn + std::to_string(i) + ".";
     F->fn_conv[i] = pack_ckc(e, ck.f32(p + "conv.weight", {256, cin, 3}), ck.f32(p + "conv.bias", {256}), 256, cin, 3);
     F->fn_g[i] = up(e, ck.f32(p + "norm.weight", {256}), 256);
@@ -1449,3 +1467,5 @@ extern "C" int ts_face_forward(ts_engine* e, const float* wave, const float* id,
   face_run(e, wave, id, out, B, N, frame, s);
   TS_API_END(e)
 }
+
+extern "C" int ts_face_dim(ts_engine* e) { return (e && e->face) ? e->face->jaw_dim + e->face->exp_dim : 0; }

@@ -249,14 +249,23 @@ class Engine:
                     "ts_vq_encode")
         return (idx, e) if want_e else idx
 
+    @property
+    def face_dim(self):
+        """output columns of the loaded face net: 103 (3-D jaw), 106 (6-D jaw, identity-free net); 0 when none is loaded."""
+        return int(self.L.ts_face_dim(self.h))
+
     def face_forward(self, wave, id_onehot, frame):
-        """s2g_face.Generator.forward: wave [B,N], id [B,4] -> [B,frame,103]."""
+        """s2g_face.Generator.forward: wave [B,N], id [B,4] -> [B,frame,face_dim].  The identity-free (6-D) net ignores id."""
         wave = self._dev(wave, torch.float32)
         B, N = wave.shape
-        idv = self._dev(id_onehot, torch.float32)
-        if idv.shape[0] == 1 and B > 1:
-            idv = idv.expand(B, -1).contiguous()
-        out = torch.empty(B, frame, 103, device=self.device)
+        D = self.face_dim
+        if D == 106:
+            idv = None
+        else:
+            idv = self._dev(id_onehot, torch.float32)
+            if idv.shape[0] == 1 and B > 1:
+                idv = idv.expand(B, -1).contiguous()
+        out = torch.empty(B, frame, D or 103, device=self.device)
         self._check(self.L.ts_face_forward(self.h, _lib.ptr(wave), _lib.ptr(idv), _lib.ptr(out), B, N, frame,
                                            self._s()), "ts_face_forward")
         return out
@@ -330,11 +339,21 @@ class Engine:
         return out
 
     def assemble_pose(self, face, body, stand=False):
-        """demo.py:182-229 + part2full: face [B,Ff,103], body [B,Fb,129] -> [B,Ff,265]."""
+        """demo.py:182-229 + part2full: face [B,Ff,103], body [B,Fb,129] -> [B,Ff,265]; or, for convert_to_6d outputs,
+        face [B,Ff,106], body [B,Fb,258] (6-D jaw / joints converted to axis-angle in the same kernel) -> [B,Ff,265]."""
         face = self._dev(face, torch.float32)
         body = self._dev(body, torch.float32)
+        if face.dim() != 3 or body.dim() != 3 or body.shape[0] != face.shape[0]:
+            raise ValueError("assemble_pose: face %s, body %s (expected [B,Ff,C] and [B,Fb,C])"
+                             % (tuple(face.shape), tuple(body.shape)))
+        dims = (face.shape[2], body.shape[2])
+        if dims == (103, 129):
+            fn, name = self.L.ts_assemble_pose, "ts_assemble_pose"
+        elif dims == (106, 258):
+            fn, name = self.L.ts_assemble_pose6d, "ts_assemble_pose6d"
+        else:
+            raise ValueError("assemble_pose: face / body columns %s: expected (103, 129) or, 6-D, (106, 258)" % (dims,))
         B, Ff, _ = face.shape
         out = torch.empty(B, Ff, 265, device=self.device)
-        self._check(self.L.ts_assemble_pose(self.h, _lib.ptr(face), _lib.ptr(body), _lib.ptr(out), B, Ff,
-                                            body.shape[1], int(stand), self._s()), "ts_assemble_pose")
+        self._check(fn(self.h, _lib.ptr(face), _lib.ptr(body), _lib.ptr(out), B, Ff, body.shape[1], int(stand), self._s()), name)
         return out

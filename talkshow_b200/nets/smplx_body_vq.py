@@ -5,7 +5,7 @@ from __future__ import annotations
 import numpy as np
 import torch
 
-from ..data_utils.lower_body import c_index_3d
+from ..data_utils.lower_body import c_index_3d, c_index_6d
 from .base import resolve_device, shared_engine, strip_module
 
 
@@ -18,17 +18,23 @@ class TrainWrapper:
         self.expression = self.config.Data.pose.expression
         self.num_classes = 4
         self.composition = self.config.Model.composition
-        if self.convert_to_6d or not self.composition:
-            raise NotImplementedError("talkshow_b200 builds the shipped config/body_vq.json geometry")
-        self.each_dim = [0, 39, 90, 100 if self.expression else 0]
-        self.c_index = c_index_3d
+        if not self.composition:
+            raise NotImplementedError("talkshow_b200 builds the composition=true VQ-VAE pair (config/body_vq.json)")
+        scale = 2 if self.convert_to_6d else 1                                   # nets/smplx_body_vq.py:96-126
+        self.each_dim = [0, 39 * scale, 90 * scale, 100 if self.expression else 0]
+        self.c_index = c_index_6d if self.convert_to_6d else c_index_3d
         self.engine = engine or shared_engine(self.device)
 
     def load_state_dict(self, state_dict):
-        """{'g_body': sd, 'g_hand': sd} (nets/smplx_body_vq.py:297-302)."""
+        """{'g_body': sd, 'g_hand': sd} (nets/smplx_body_vq.py:297-302).  Like the reference's strict load, VQ-VAEs whose
+        pose channels are not the config's (39 / 90, or 78 / 180 with convert_to_6d) raise RuntimeError."""
         self._loaded = {"g_body": strip_module(state_dict["g_body"]), "g_hand": strip_module(state_dict["g_hand"])}
         self.engine.load_vq(0, self._loaded["g_body"])
         self.engine.load_vq(1, self._loaded["g_hand"])
+        got = [self.engine.vq_dim(0), self.engine.vq_dim(1)]
+        if got != self.each_dim[1:3]:
+            raise RuntimeError("s2g_body_vq: the checkpoint's VQ-VAEs have %s pose channels, the config (convert_to_6d=%s) "
+                               "builds %s" % (got, self.convert_to_6d, self.each_dim[1:3]))
 
     def state_dict(self):
         """nets/smplx_body_vq.py:77-94 (composition): the loaded weights in the layout the reference saves; optimizer and
@@ -38,17 +44,21 @@ class TrainWrapper:
                 "discriminator": None, "discriminator_optim": None}
 
     def encode(self, initial_pose):
-        """initial_pose (B,165,F) -> (idx_body [B,T], idx_hand [B,T]) int64 on the device."""
+        """initial_pose (B,165,F), (B,330,F) with convert_to_6d -> (idx_body [B,T], idx_hand [B,T]) int64 on the device."""
         gt = initial_pose.to(torch.float32)[:, self.c_index].permute(0, 2, 1).contiguous()
-        ib = self.engine.vq_encode(0, gt[..., :39].contiguous())
-        ih = self.engine.vq_encode(1, gt[..., 39:].contiguous())
+        nb = self.each_dim[1]
+        ib = self.engine.vq_encode(0, gt[..., :nb].contiguous())
+        ih = self.engine.vq_encode(1, gt[..., nb:].contiguous())
         return ib, ih
 
     def infer_on_audio(self, aud_fn, initial_pose=None, norm_stats=None, exp=None, var=None, w_pre=False,
                        continuity=False, id=None, fps=15, sr=22000, smooth=False, **kwargs):
-        """initial_pose (B,165,F) -> numpy (F, B*129) (nets/smplx_body_vq.py:208-295; the audio
+        """initial_pose (B,165,F) -> numpy (F, B*129); (B,330,F) -> (F, B*258) with convert_to_6d
+        (nets/smplx_body_vq.py:208-295; the audio
         argument is unused by the reference's VQ path too)."""
         assert self.args.infer, "train mode"
+        if self.config.Data.pose.normalization:
+            raise NotImplementedError("normalised VQ outputs are outside the built path (config/body_vq.json: false)")
         if continuity:
             # :256-271: five 60-frame chunks, each encoded/quantised/decoded on its own (pre_state is ignored by
             # Decoder.forward, vqvae_1d.py:139-149) and concatenated along time
@@ -62,7 +72,7 @@ class TrainWrapper:
             ib, ih = self.encode(initial_pose)
             body = self.engine.vq_decode(0, ib)
             hand = self.engine.vq_decode(1, ih)
-        output = torch.cat([body, hand], 1).transpose(1, 2).cpu().numpy()          # (B,F,129)
+        output = torch.cat([body, hand], 1).transpose(1, 2).cpu().numpy()          # (B,F,129) / (B,F,258)
         if smooth:                                                                  # :283-291
             lamda, smooth_f, frame = 0.8, 10, 149
             for i in range(smooth_f):

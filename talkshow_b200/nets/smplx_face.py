@@ -1,5 +1,6 @@
 """s2g_face — host mirror of nets/smplx_face.py (inference): raw 16 kHz waveform -> jaw(3) +
-expression(100) per 30 fps frame, through the wav2vec2-based regressor in the CUDA engine."""
+expression(100) per 30 fps frame, through the wav2vec2-based regressor in the CUDA engine.  With convert_to_6d the
+reference builds the identity-free net (identity=False) with a 6-D jaw head: jaw(6) + expression(100)."""
 from __future__ import annotations
 
 import torch
@@ -45,16 +46,27 @@ class TrainWrapper:
         self.convert_to_6d = self.config.Data.pose.convert_to_6d
         self.expression = self.config.Data.pose.expression
         self.num_classes = 4
+        # nets/smplx_face.py:63-93 (init_params, scale 2 for 6-D); the 6-D net has no id_mlp (:37-45, identity=False)
         if self.convert_to_6d:
-            raise NotImplementedError("talkshow_b200 builds the shipped config/face.json geometry (3-D jaw)")
-        self.each_dim = [3, 75, 90, 100 if self.expression else 0]        # nets/smplx_face.py:63-93
-        self.dim_list = [0, 3, 9, 75, 165]
+            self.each_dim = [6, 144, 180, 100 if self.expression else 0]
+            self.dim_list = [0, 6, 18, 150, 330]
+        else:
+            self.each_dim = [3, 75, 90, 100 if self.expression else 0]
+            self.dim_list = [0, 3, 9, 75, 165]
         self.engine = engine or shared_engine(self.device)
 
     def load_state_dict(self, state_dict):
-        """ckpt['generator'] of a face checkpoint: {'generator': Generator sd, ...} (nets/base.py:38-54)."""
-        sd = state_dict["generator"] if "generator" in state_dict else state_dict
-        self._loaded = strip_module(sd)
+        """ckpt['generator'] of a face checkpoint: {'generator': Generator sd, ...} (nets/base.py:38-54).  Like the
+        reference's strict load, a checkpoint whose output geometry is not the config's raises RuntimeError."""
+        sd = strip_module(state_dict["generator"] if "generator" in state_dict else state_dict)
+        got = [int(sd[k].shape[0]) if k in sd else 0 for k in ("final_out.0.weight", "final_out.1.weight")]
+        identity = "audio_middle.id_mlp.weight" in sd
+        if got != [self.each_dim[0], self.each_dim[3]] or identity == self.convert_to_6d:
+            raise RuntimeError("s2g_face: the checkpoint's net (jaw %d + expression %d columns, %s) is not the one the config "
+                               "builds (convert_to_6d=%s: jaw %d + expression %d, %s)"
+                               % (got[0], got[1], "id_mlp" if identity else "identity-free", self.convert_to_6d,
+                                  self.each_dim[0], self.each_dim[3], "identity-free" if self.convert_to_6d else "id_mlp"))
+        self._loaded = sd
         self.engine.load_face(self._loaded)
         self.encoder_layers = len({k.split(".")[3] for k in self._loaded if k.startswith("audio_encoder.encoder.layers.")})
 
@@ -65,7 +77,7 @@ class TrainWrapper:
 
     def infer_on_audio(self, aud_fn, id=None, initial_pose=None, norm_stats=None, w_pre=False, frame=None, am=None,
                        am_sr=16000, **kwargs):
-        """wav path or tensor [B,1,N] -> numpy (B, frame, 103) (nets/smplx_face.py:169-218)."""
+        """wav path or tensor [B,1,N] -> numpy (B, frame, 103), (B, frame, 106) with convert_to_6d (nets/smplx_face.py:169-218)."""
         if self.config.Data.pose.normalization:
             raise NotImplementedError("normalised face outputs are outside the built path (config/face.json: false)")
         B = 1 if initial_pose is None else initial_pose.shape[0]
@@ -95,6 +107,6 @@ class TrainWrapper:
         return self.engine.face_forward(wave, idv, frame)
 
     def generate(self, wv2_feat, frame):
-        """tensor API (:221-238): wv2_feat [B,1,N] -> torch (B, frame, 103); id = zeros."""
+        """tensor API (:221-238): wv2_feat [B,1,N] -> torch (B, frame, 103 or 106); id = zeros."""
         wave = wv2_feat.to(torch.float32).reshape(wv2_feat.shape[0], -1)
         return self.generate_ids(wave, torch.zeros(wave.shape[0], self.num_classes), frame)

@@ -123,10 +123,12 @@ W2V_CONV_KERNEL = (10, 3, 3, 3, 3, 2, 2)
 W2V_CONV_STRIDE = (5, 2, 2, 2, 2, 2, 2)
 
 
-def face_schema(n_classes=4, jaw_dim=3, exp_dim=100):
+def face_schema(n_classes=4, jaw_dim=3, exp_dim=100, identity=True):
     """s2g_face.Generator (nets/spg/s2g_face.py:142-194) with the HF wav2vec2-base encoder
     (transformers Wav2Vec2Model; names of the installed 5.x version, where the positional conv
-    carries a weight_norm parametrisation ``parametrizations.weight.original{0,1}`` = (g, v))."""
+    carries a weight_norm parametrisation ``parametrizations.weight.original{0,1}`` = (g, v)).
+    ``identity=False`` is the convert_to_6d net (nets/smplx_face.py:37-45): AudioEncoder(256, 256, identity=False)
+    has no id_mlp, and first_net layer 0 maps 256 -> 256 with an nn.Identity residual (nets/layers.py:95-96)."""
     s = OrderedDict()
     a = "audio_encoder."
     s[a + "masked_spec_embed"] = (768,)
@@ -160,12 +162,13 @@ def face_schema(n_classes=4, jaw_dim=3, exp_dim=100):
         s[p + "final_layer_norm.bias"] = (768,)
     s["audio_feature_map.weight"] = (256, 768)
     s["audio_feature_map.bias"] = (256,)
-    s["audio_middle.id_mlp.weight"] = (64, n_classes, 1)
-    s["audio_middle.id_mlp.bias"] = (64,)
     f = "audio_middle.first_net.conv_layers."
-    s[f + "0.residual_layer.0.weight"] = (256, 320, 3)
-    s[f + "0.residual_layer.0.bias"] = (256,)
-    for i, cin in enumerate((320, 256, 256)):
+    if identity:
+        s["audio_middle.id_mlp.weight"] = (64, n_classes, 1)
+        s["audio_middle.id_mlp.bias"] = (64,)
+        s[f + "0.residual_layer.0.weight"] = (256, 320, 3)
+        s[f + "0.residual_layer.0.bias"] = (256,)
+    for i, cin in enumerate((320 if identity else 256, 256, 256)):
         s[f + "%d.conv.weight" % i] = (256, cin, 3)
         s[f + "%d.conv.bias" % i] = (256,)
         s[f + "%d.norm.weight" % i] = (256,)
@@ -291,6 +294,11 @@ def body_vq_checkpoint(seed=0):
 
 def face_checkpoint(seed=0):
     return {"generator": face_state(seed + 4)}
+
+
+def face_checkpoint_6d(seed=0):
+    """convert_to_6d face (nets/smplx_face.py:37-45, init_params scale 2): identity-free net, 6-D jaw head."""
+    return {"generator": synth_state(face_schema(identity=False, jaw_dim=6), seed + 24)}
 
 
 def fingerprint(sd):
