@@ -108,6 +108,25 @@ int ts_vq_encode(ts_engine* e, int which, const float* poses, int64_t* idx, floa
 int ts_face_forward(ts_engine* e, const float* wave, const float* id, float* out, int B, int N, int frame,
                     void* stream);
 
+/* ---- held-out scoring: the forward half of the reference's training steps, losses kept per clip ---------------
+ * Reductions run in a fixed order without atomics (repeated calls give the same bits): elementwise terms in fp32 as the
+ * reference forms them, accumulated in fp64; clip_out is fp64.
+ *
+ * VQVAE of s2g_body_vq.vq_train + get_loss (nets/smplx_body_vq.py:155-206) in eval mode: poses [B,F,C] (C = ts_vq_dim)
+ * -> encoder + argmin (idx_out [B,T], T = F/4, bit-identical to ts_vq_encode) -> decoder on the quantised embeddings
+ * (recon_out, may be NULL, [B,F,C], bit-identical to ts_vq_decode of those indices, transposed) and per clip
+ * clip_out [B,3] = { sum |recon - gt| over (F,C), sum |d recon - d gt| over (F-1,C) (d = frame-to-frame difference),
+ * sum ||z - e[idx]||^2 over the T latent rows (z = encoder output before quantisation) }.
+ * F must be a positive multiple of 4 (otherwise TS_ERR_INVALID: the reference fails on the recon / gt shape mismatch). */
+int ts_vq_score(ts_engine* e, int which, const float* poses, int64_t* idx_out, float* recon_out, double* clip_out, int B,
+                int F, void* stream);
+/* s2g_face.__call__ + get_loss (nets/smplx_face.py:95-167) in eval mode, frame = F: the ts_face_forward computation
+ * (pred_out, may be NULL, [B,F,ts_face_dim], bit-identical to it) against gt [B,F,Cgt] (Cgt >= 100: pose columns then
+ * the 100 expression columns) -> clip_out [B,2] = { sum |pred[:,:,:6] - gt[:,:,:6]|, sum (pred[:,:,-100:] - gt[:,:,-100:])^2 }.
+ * Either net: id [B,4] is required by the identity net (103 columns) and may be NULL for the identity-free one (106). */
+int ts_face_score(ts_engine* e, const float* wave, const float* id, const float* gt, int Cgt, float* pred_out,
+                  double* clip_out, int B, int N, int F, void* stream);
+
 /* output columns of the loaded face net: 103 (jaw 3 + expression 100) or 106 (6-D jaw 6 + expression 100);
  * 0 when no face is loaded. */
 int ts_face_dim(ts_engine* e);

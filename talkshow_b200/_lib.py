@@ -57,6 +57,10 @@ SYMBOLS = {
     "ts_assemble_pose6d": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                      C.c_int, C.c_void_p]),
     "ts_face_dim": (C.c_int, [C.c_void_p]),
+    "ts_vq_score": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                              C.c_void_p]),
+    "ts_face_score": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+                                C.c_int, C.c_int, C.c_void_p]),
     "ts_mfcc": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "ts_mfcc_frames": (C.c_int, [C.c_int, C.c_int]),
     "ts_launch_count": (C.c_int64, [C.c_void_p]),

@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libtalkshow_b200.so")
-SOURCES = ["api.cu", "gemm.cu", "gemm_tc.cu", "convstack.cu", "pixelcnn.cu", "pixelcnn_tf.cu", "face.cu", "mfcc.cu", "lbs.cu", "collective.cu"]
+SOURCES = ["api.cu", "gemm.cu", "gemm_tc.cu", "convstack.cu", "pixelcnn.cu", "pixelcnn_tf.cu", "face.cu", "score.cu", "mfcc.cu", "lbs.cu", "collective.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]

@@ -243,17 +243,6 @@ Act3 run_vq_decode(ts_engine* e, const VQNet& v, const int64_t* idx, int B, int 
 
 using namespace ts;
 
-// sizing pass + real pass over the same code path
-template <class F>
-static void run_sized(ts_engine* e, F&& body) {
-  e->ws.begin_sizing();
-  body();
-  size_t need = e->ws.need;
-  e->ws.buf.ensure(need + 256);
-  e->ws.begin(need);
-  body();
-}
-
 extern "C" int ts_latent_rows(int M) {
   int m = (M + 2 - 4) / 2 + 1;
   return (m + 2 - 4) / 2 + 1;

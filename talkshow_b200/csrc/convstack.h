@@ -38,4 +38,15 @@ Act3 run_trunk(ts_engine* e, const Trunk& t, const Act3& x, cudaStream_t s);
 Act3 run_decoder(ts_engine* e, const VQNet& v, const Act3& q, cudaStream_t s);
 Act3 run_vq_decode(ts_engine* e, const VQNet& v, const int64_t* idx, int B, int T, cudaStream_t s);
 
+// sizing pass + real pass over the same code path
+template <class F>
+void run_sized(ts_engine* e, F&& body) {
+  e->ws.begin_sizing();
+  body();
+  size_t need = e->ws.need;
+  e->ws.buf.ensure(need + 256);
+  e->ws.begin(need);
+  body();
+}
+
 }  // namespace ts

@@ -1244,7 +1244,9 @@ static void linear(ts_engine* e, const Layer& L, const Act3& x, const Act3& y, i
   conv_auto(e, L, x, 1, 1, 0, y, x.T, act, res, s, 1, 0, coff);
 }
 
-static void face_run(ts_engine* e, const float* wave, const float* idv, float* out, int B, int N, int frame, cudaStream_t s) {
+bool face_has_identity(const ts_engine* e) { return e->face && e->face->identity; }
+
+void face_run(ts_engine* e, const float* wave, const float* idv, float* out, int B, int N, int frame, cudaStream_t s) {
   FaceNet& F = *e->face;
   // ---- wav2vec2 feature extractor ---------------------------------------------------------
   int T = (N - 10) / 5 + 1;

@@ -82,6 +82,10 @@ void pixel_destroy(ts_engine* e);
 void* tf_build(ts_engine* e, const Ckpt& ck, int L, int D, int ncls);
 void tf_free(void* p);
 void face_destroy(ts_engine* e);
+// face.cu: s2g_face.Generator.forward into out [B,frame,ts_face_dim] (workspace from e->ws, sizing-pass aware), and
+// whether the loaded net is the identity net (reads id)
+void face_run(ts_engine* e, const float* wave, const float* idv, float* out, int B, int N, int frame, cudaStream_t s);
+bool face_has_identity(const ts_engine* e);
 void mfcc_destroy(ts_engine* e);
 void smplx_destroy(ts_engine* e);
 void nccl_destroy(ts_engine* e);

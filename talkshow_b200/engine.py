@@ -249,6 +249,49 @@ class Engine:
                     "ts_vq_encode")
         return (idx, e) if want_e else idx
 
+    def vq_score(self, which, poses, want_recon=False):
+        """Held-out VQ-VAE score (vq_train + get_loss, eval): poses [B,F,C] (C = vq_dim, F % 4 == 0) -> (idx [B,T],
+        clip [B,3] float64 = per-clip sums of |recon - gt|, |d recon - d gt| and ||z - e[idx]||^2, recon [B,F,C] or None).
+        idx equals vq_encode's, recon equals vq_decode(idx) transposed."""
+        poses = self._dev(poses, torch.float32)
+        C_ = self.vq_dim(which)
+        if poses.dim() != 3 or poses.shape[2] != C_ or poses.shape[0] < 1 or poses.shape[1] < 4 or poses.shape[1] % 4:
+            raise ValueError("vq_score: poses %s (expected [B,F,%d] with F a positive multiple of 4)"
+                             % (tuple(poses.shape), C_))
+        B, F_, _ = poses.shape
+        idx = torch.empty(B, F_ // 4, dtype=torch.int64, device=self.device)
+        clip = torch.empty(B, 3, dtype=torch.float64, device=self.device)
+        recon = torch.empty(B, F_, C_, device=self.device) if want_recon else None
+        self._check(self.L.ts_vq_score(self.h, which, _lib.ptr(poses), _lib.ptr(idx), _lib.ptr(recon), _lib.ptr(clip), B, F_,
+                                       self._s()), "ts_vq_score")
+        return idx, clip, recon
+
+    def face_score(self, wave, id_onehot, gt, want_pred=False):
+        """Held-out face score (__call__ + get_loss, eval, frame = F): wave [B,N], id [B,4], gt [B,F,Cgt] (pose columns,
+        then the 100 expression columns) -> (clip [B,2] float64 = per-clip sums of |pred[..,:6] - gt[..,:6]| and
+        (pred[..,-100:] - gt[..,-100:])^2, pred [B,F,face_dim] or None).  pred equals face_forward(wave, id, F)."""
+        wave = self._dev(wave, torch.float32)
+        gt = self._dev(gt, torch.float32)
+        D = self.face_dim
+        if wave.dim() != 2 or gt.dim() != 3 or gt.shape[0] != wave.shape[0] or gt.shape[2] < 100 or gt.shape[1] < 1:
+            raise ValueError("face_score: wave %s, gt %s (expected [B,N] and [B,F,C] with C >= 100)"
+                             % (tuple(wave.shape), tuple(gt.shape)))
+        B, N = wave.shape
+        F_ = gt.shape[1]
+        if D == 106:
+            idv = None
+        else:
+            idv = self._dev(id_onehot, torch.float32)
+            if idv.shape[0] == 1 and B > 1:
+                idv = idv.expand(B, -1).contiguous()
+            if tuple(idv.shape) != (B, 4):
+                raise ValueError("face_score: id %s (expected [B,4])" % (tuple(idv.shape),))
+        clip = torch.empty(B, 2, dtype=torch.float64, device=self.device)
+        pred = torch.empty(B, F_, D or 103, device=self.device) if want_pred else None
+        self._check(self.L.ts_face_score(self.h, _lib.ptr(wave), _lib.ptr(idv), _lib.ptr(gt), gt.shape[2], _lib.ptr(pred),
+                                         _lib.ptr(clip), B, N, F_, self._s()), "ts_face_score")
+        return clip, pred
+
     @property
     def face_dim(self):
         """output columns of the loaded face net: 103 (3-D jaw), 106 (6-D jaw, identity-free net); 0 when none is loaded."""

@@ -9,6 +9,40 @@ from ..data_utils.lower_body import c_index_3d, c_index_6d
 from .base import resolve_device, shared_engine, strip_module
 
 
+COMMITMENT_COST = 0.25   # VQVAE(..., commitment_cost=0.25), nets/spg/vqvae_1d.py:171-181
+
+
+def score_vq_pair(engine, gt, n_body):
+    """vq_train + get_loss of the body and the hand VQ-VAE (nets/smplx_body_vq.py:145-148,155-206) in eval mode.
+    gt [B,F,C] (c_index applied; body columns first, n_body of them) ->
+    (codes [B,T,2], {'brec_loss', 'bvelocity_loss', 'hrec_loss', 'hvelocity_loss'} as floats, per-clip float64 values of
+    those four and of 'be_q_loss' / 'he_q_loss' = commitment_cost * mean ||z - e||^2, the term the reference leaves out
+    of its dict)."""
+    B, F = gt.shape[:2]
+    losses, per_clip, codes = {}, {}, []
+    for name, which, part in (("b", 0, gt[..., :n_body]), ("h", 1, gt[..., n_body:])):
+        idx, clip, _ = engine.vq_score(which, part.contiguous())
+        clip = clip.cpu()
+        C, T = part.shape[2], idx.shape[1]
+        per_clip[name + "rec_loss"] = clip[:, 0] / (F * C)
+        per_clip[name + "velocity_loss"] = clip[:, 1] / ((F - 1) * C)
+        per_clip[name + "e_q_loss"] = COMMITMENT_COST * clip[:, 2] / (T * 64)
+        losses[name + "rec_loss"] = float(clip[:, 0].sum() / (B * F * C))
+        losses[name + "velocity_loss"] = float(clip[:, 1].sum() / (B * (F - 1) * C))
+        codes.append(idx)
+    return torch.stack(codes, -1), losses, per_clip
+
+
+def check_pose_block(poses, convert_to_6d, who):
+    """[B,165,F] (axis-angle) or [B,330,F] (convert_to_6d) with F a positive multiple of 4, else ValueError."""
+    rows = 330 if convert_to_6d else 165
+    if poses.dim() != 3 or poses.shape[1] != rows:
+        raise ValueError("%s: poses %s, expected [B,%d,F] (convert_to_6d=%s)" % (who, tuple(poses.shape), rows, convert_to_6d))
+    if poses.shape[2] < 4 or poses.shape[2] % 4:
+        # the decoder returns 4 * (latent rows) frames: the reference fails on the recon / gt shape mismatch
+        raise ValueError("%s: %d pose frames, the VQ-VAE scores multiples of 4" % (who, poses.shape[2]))
+
+
 class TrainWrapper:
     def __init__(self, args, config, engine=None):
         self.args = args
@@ -42,6 +76,19 @@ class TrainWrapper:
         loaded = getattr(self, "_loaded", {"g_body": None, "g_hand": None})
         return {"g_body": loaded["g_body"], "g_body_optim": None, "g_hand": loaded["g_hand"], "g_hand_optim": None,
                 "discriminator": None, "discriminator_optim": None}
+
+    def evaluate(self, bat):
+        """The forward half of the reference's training step __call__(bat) (:128-206) in eval mode, which the reference
+        itself cannot run (in eval VQVAE.forward returns (e, recon) untransposed and get_loss fails): encoder -> argmin
+        quantisation -> decoder on the codebook rows (no straight-through add) -> get_loss.  bat: 'poses' [B,165,F], or
+        [B,330,F] with convert_to_6d; F a multiple of 4.  Returns (None, {'brec_loss', 'bvelocity_loss', 'hrec_loss',
+        'hvelocity_loss'}); per-clip values, the commitment terms included, are kept as self.last_losses and the codes
+        [B,T,2] as self.last_codes."""
+        poses = torch.as_tensor(bat["poses"]).to(torch.float32)
+        check_pose_block(poses, self.convert_to_6d, "s2g_body_vq.evaluate")
+        gt = poses[:, self.c_index, :].permute(0, 2, 1)
+        self.last_codes, losses, self.last_losses = score_vq_pair(self.engine, gt, self.each_dim[1])
+        return None, losses
 
     def encode(self, initial_pose):
         """initial_pose (B,165,F), (B,330,F) with convert_to_6d -> (idx_body [B,T], idx_hand [B,T]) int64 on the device."""

@@ -32,6 +32,26 @@ def hf_layerdrop_uses_torch_rng():
     return _HF_TORCH_LAYERDROP
 
 
+def face_gt(poses, expression):
+    """__call__'s target (:107-111): poses [B,C,F] and expression [B,100,F] -> [B,F,C+100]."""
+    poses, expression = poses.to(torch.float32), expression.to(torch.float32)
+    if poses.dim() != 3 or expression.dim() != 3 or expression.shape[1] != 100 or poses.shape[0] != expression.shape[0] \
+            or poses.shape[2] != expression.shape[2]:
+        raise ValueError("face evaluate: poses %s, expression %s (expected [B,C,F] and [B,100,F])"
+                         % (tuple(poses.shape), tuple(expression.shape)))
+    return torch.cat([poses.permute(0, 2, 1), expression.permute(0, 2, 1)], 2)
+
+
+def score_face(engine, wave, idv, gt):
+    """get_loss (:139-167) of the regressor's prediction at frame = F against gt [B,F,C] ->
+    ({'MSELoss', 'exp_loss'} as floats, the same two per clip as float64 tensors)."""
+    B, F_ = gt.shape[:2]
+    clip, _ = engine.face_score(wave, idv, gt)
+    clip = clip.cpu()
+    per_clip = {"MSELoss": clip[:, 0] / (F_ * 6), "exp_loss": clip[:, 1] / (F_ * 100)}
+    return {"MSELoss": float(clip[:, 0].sum() / (B * F_ * 6)), "exp_loss": float(clip[:, 1].sum() / (B * F_ * 100))}, per_clip
+
+
 class TrainWrapper:
     # torch.rand([]) draws consumed from the default CPU generator per forward, so that a seeded run of the demo flow samples
     # the same body codes as the reference does in the same environment.  None: what the reference would consume with the
@@ -74,6 +94,28 @@ class TrainWrapper:
         """nets/base.py:29-36: {'generator': ..., optimizer / discriminator slots empty}."""
         return {"generator": getattr(self, "_loaded", None), "generator_optim": None, "discriminator": None,
                 "discriminator_optim": None}
+
+    def evaluate(self, bat):
+        """The forward half of the reference's training step __call__(bat) (:95-167) in eval mode.  bat: 'aud_feat'
+        [B,1,N] (the 16 kHz waveform; permuted and flattened to [B,N] as :106 does), 'poses' [B,C,F], 'expression'
+        [B,100,F], 'speaker' [B] (id = one_hot(speaker - 20)).  Returns (None, {'MSELoss', 'exp_loss'}); per-clip values
+        are kept as self.last_losses.  Kept from the reference, on purpose:
+          - 'MSELoss' is an L1 over the first 6 columns in both geometries (on the 3-D net: the jaw and the first three
+            expression columns of the prediction, against the first 6 columns of poses);
+          - the reference sets time_steps = F only in training mode; the regressor runs with frame = F here;
+          - 'grad' is not reported: there is no backward pass.
+        It consumes the same torch.rand([]) draws as generate_ids."""
+        if not self.expression:
+            raise NotImplementedError("the face regressor is built with its expression head (config/face.json)")
+        aud = torch.as_tensor(bat["aud_feat"]).to(torch.float32)
+        wave = aud.permute(0, 2, 1).reshape(aud.shape[0], -1)
+        gt = face_gt(torch.as_tensor(bat["poses"]), torch.as_tensor(bat["expression"]))
+        if gt.shape[0] != wave.shape[0]:
+            raise ValueError("face evaluate: %d waveforms for %d pose clips" % (wave.shape[0], gt.shape[0]))
+        idv = F.one_hot((torch.as_tensor(bat["speaker"]) - 20).reshape(-1).to(torch.int64), self.num_classes).to(torch.float32)
+        self._mirror_reference_rng()
+        losses, self.last_losses = score_face(self.engine, wave, idv, gt)
+        return None, losses
 
     def infer_on_audio(self, aud_fn, id=None, initial_pose=None, norm_stats=None, w_pre=False, frame=None, am=None,
                        am_sr=16000, **kwargs):

@@ -105,6 +105,39 @@ class WholeBody:
         _, body = self.e.body_generate(mfcc, label, noise, want_codes=False)
         return self.e.assemble_pose(face, body, stand)
 
+    def evaluate(self, bat):
+        """Score held-out clips under the loaded face / VQ / prior trio: what s2g_face.evaluate, s2g_body_vq.evaluate and
+        s2g_body_pixel.evaluate return, in one call, with the VQ encoder run once (the codes of the VQ score feed the prior
+        score).  bat: 'wave' [B,N] (16 kHz, the face input), 'aud_feat' [B,64,M] (MFCC), 'poses' [B,165,F] ([B,330,F] for a
+        convert_to_6d trio), 'expression' [B,100,F], 'speaker' [B].  F must be a multiple of 4 and M must give F/4 latent
+        rows.  Returns (None, {'MSELoss', 'exp_loss', 'brec_loss', 'bvelocity_loss', 'hrec_loss', 'hvelocity_loss',
+        'ce_loss'}); per-clip values are kept as self.last_losses, the per-position prior NLL as self.last_nll."""
+        import torch.nn.functional as F
+
+        from .data_utils.lower_body import c_index_3d, c_index_6d
+        from .nets.smplx_body_vq import check_pose_block, score_vq_pair
+        from .nets.smplx_face import face_gt, score_face
+
+        six = self.e.vq_dim(0) == 78
+        poses = torch.as_tensor(bat["poses"]).to(torch.float32)
+        check_pose_block(poses, six, "WholeBody.evaluate")
+        mfcc = torch.as_tensor(bat["aud_feat"]).to(torch.float32)
+        B, nf = poses.shape[0], poses.shape[2]
+        if mfcc.dim() != 3 or mfcc.shape[0] != B or self.e.latent_rows(mfcc.shape[2]) != nf // 4:
+            # the reference fails in the prior's concatenation of code and audio rows (gated_pixelcnn_v2.py:143)
+            raise ValueError("WholeBody.evaluate: aud_feat %s gives %d latent rows, %d pose frames give %d"
+                             % (tuple(mfcc.shape), self.e.latent_rows(mfcc.shape[2]) if mfcc.dim() == 3 else -1, nf, nf // 4))
+        wave = torch.as_tensor(bat["wave"]).to(torch.float32).reshape(B, -1)
+        label = (torch.as_tensor(bat["speaker"]) - 20).reshape(-1).to(torch.int64)
+        face_losses, face_clip = score_face(self.e, wave, F.one_hot(label, 4).to(torch.float32),
+                                            face_gt(poses, torch.as_tensor(bat["expression"])))
+        gt = poses[:, c_index_6d if six else c_index_3d, :].permute(0, 2, 1)
+        codes, vq_losses, vq_clip = score_vq_pair(self.e, gt, 78 if six else 39)
+        nll = self.e.pixelcnn_score(self.e.audio_encode(mfcc), label, codes)
+        self.last_nll = nll
+        self.last_losses = dict(face_clip, **vq_clip)
+        return None, dict(face_losses, **vq_losses, ce_loss=float(nll.double().mean()))
+
     def generate_sharded(self, mfcc, wave, label, rank, world, noise_full=None, seed=None, stand=False, gather=True,
                          group=None):
         """Multi-GPU form of ``generate`` whose RESULT DOES NOT DEPEND ON ``world`` (SURVEY.md §8e): the arguments are
