@@ -81,6 +81,24 @@ int ts_latent_rows(int M);
 int ts_pixelcnn_generate(ts_engine* e, const float* aud, const int64_t* label, const float* noise,
                          int64_t* idx_out, float* logits_out, int B, int T, const int64_t* pre_latents, int T0,
                          void* stream);
+/* ts_pixelcnn_generate with sampling controls.  Let l be the 2048 raw logits of one draw (what logits_out holds).
+ *  - top_k (0 = off, 1..2048): keep code i iff l_i >= v_k, v_k the k-th largest logit counting multiplicity (ties at the
+ *    boundary are all kept; TopKLogitsWarper).  The comparison is on the raw logits, whatever the temperature.
+ *  - temperature > 0: s = l / temperature (IEEE division), dropped codes -> -inf, then the default draw on s:
+ *    argmax(softmax(s) / q) with first-index ties, same noise and RNG contract.  A dropped code is never drawn, even when
+ *    every kept probability underflows to 0.  Any finite temperature > 0 is valid: one so small that max l / temperature
+ *    overflows (e.g. a subnormal temperature) leaves every tempered probability NaN, and the code is then the greedy one,
+ *    the limit of the tempered draw as the temperature goes to 0.  Codes always lie in [0, 2048).
+ *  - temperature = 0 (greedy): code = first index of max l.  noise is not read and may be NULL.
+ *  - logp_out (may be NULL) [B,T,2], laid out like idx_out: log_softmax(l)[code] of the untempered, untruncated model
+ *    (= -nll of ts_pixelcnn_score), computed as (l[code] - max l) - logf(sum exp(l - max l)).  Rows forced by
+ *    pre_latents have no entry.
+ * temperature 1 with top_k 0 or 2048 gives codes bit-identical to ts_pixelcnn_generate.  The launches are those of
+ * ts_pixelcnn_generate.  TS_ERR_INVALID: temperature < 0 or not finite, top_k outside [0, 2048], NULL noise with
+ * temperature > 0. */
+int ts_pixelcnn_sample(ts_engine* e, const float* aud, const int64_t* label, const float* noise,
+                       int64_t* idx_out, float* logits_out, int B, int T, const int64_t* pre_latents, int T0,
+                       float temperature, int top_k, float* logp_out, void* stream);
 /* GatedPixelCNN.forward (teacher forced), :130-150, for rows [0,T): logits_out [B,2048,T,2]. */
 int ts_pixelcnn_logits(ts_engine* e, const float* aud, const int64_t* label, const int64_t* codes,
                        float* logits_out, int B, int T, void* stream);
@@ -140,6 +158,10 @@ int ts_vq_dim(ts_engine* e, int which);
  * (body 39 + hand 90 = 129; 258 for the 6-D configs). */
 int ts_body_generate(ts_engine* e, const float* mfcc, const int64_t* label, const float* noise, int64_t* codes,
                      float* poses, int B, int M, void* stream);
+/* ts_body_generate with the sampling controls of ts_pixelcnn_sample (same semantics, same error statuses):
+ * temperature, top_k, logp_out [B,T,2] (may be NULL); noise may be NULL when temperature = 0. */
+int ts_body_sample(ts_engine* e, const float* mfcc, const int64_t* label, const float* noise, int64_t* codes,
+                   float* poses, int B, int M, float temperature, int top_k, float* logp_out, void* stream);
 
 /* Audio front-end of get_mfcc_ta, data_utils/utils.py:148-177 (SURVEY.md §8f-1): wave [B,N] mono at
  * `sr` Hz -> torchaudio Resample(sr, 22000) -> MFCC(64 coefficients, n_fft 2048, hop 734 = 30 fps, 256 HTK

@@ -42,6 +42,10 @@ SYMBOLS = {
     "ts_smplx_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "ts_pixelcnn_generate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p]),
+    "ts_pixelcnn_sample": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                     C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_void_p, C.c_void_p]),
+    "ts_body_sample": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                 C.c_int, C.c_float, C.c_int, C.c_void_p, C.c_void_p]),
     "ts_pixelcnn_logits": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                      C.c_void_p]),
     "ts_pixelcnn_score": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,

@@ -239,9 +239,9 @@ extern "C" int ts_vq_dim(ts_engine* e, int which) {
 }
 
 // ---- fused body path: audio encoder -> PixelCNN sampler -> two VQ decoders -------------------------
-extern "C" int ts_body_generate(ts_engine* e, const float* mfcc, const int64_t* label, const float* noise,
-                                int64_t* codes, float* poses, int B, int M, void* stream) {
-  TS_API_BEGIN(e)
+// ctl = nullptr: the default sampler (ts_body_generate); else the sampling controls of ts_body_sample
+static void body_generate(ts_engine* e, const float* mfcc, const int64_t* label, const float* noise, int64_t* codes,
+                          float* poses, int B, int M, void* stream, const SampleCtl* ctl) {
   ts::require_device(e);
   if (!e->conv || !e->conv->audio_loaded) fail(TS_ERR_NOT_LOADED, "audio encoder weights not loaded");
   if (!e->conv->vq[0].loaded || !e->conv->vq[1].loaded) fail(TS_ERR_NOT_LOADED, "vq weights not loaded");
@@ -258,7 +258,7 @@ extern "C" int ts_body_generate(ts_engine* e, const float* mfcc, const int64_t* 
     Act3 a = run_trunk(e, e->conv->audio, x, s);          // [B,T,256] channel-last, pad 1
     int64_t* idx = e->ws.alloc<int64_t>((size_t)B * T * 2);
     int64_t* idx_c = e->ws.alloc<int64_t>((size_t)B * T * 2);  // [2][B][T] column-split copy
-    pixelcnn_generate_act(e, a, label, noise, idx, nullptr, B, T, nullptr, 0, s);
+    pixelcnn_generate_act(e, a, label, noise, idx, nullptr, B, T, nullptr, 0, s, false, ctl);
     split_codes(e, idx, idx_c, B, T, codes, s);
     const int c0 = e->conv->vq[0].out_dim, c1 = e->conv->vq[1].out_dim;   // 39 + 90 (axis-angle) or 78 + 180 (6-D)
     // Small batches: each decoder is a chain of ~20 launches that fill a few SMs, so the hand decoder runs on a second
@@ -292,5 +292,21 @@ extern "C" int ts_body_generate(ts_engine* e, const float* mfcc, const int64_t* 
   e->ws.buf.ensure(need + 256);
   e->ws.begin(need);
   body();
+}
+
+extern "C" int ts_body_generate(ts_engine* e, const float* mfcc, const int64_t* label, const float* noise,
+                                int64_t* codes, float* poses, int B, int M, void* stream) {
+  TS_API_BEGIN(e)
+  body_generate(e, mfcc, label, noise, codes, poses, B, M, stream, nullptr);
+  TS_API_END(e)
+}
+
+extern "C" int ts_body_sample(ts_engine* e, const float* mfcc, const int64_t* label, const float* noise, int64_t* codes,
+                              float* poses, int B, int M, float temperature, int top_k, float* logp_out, void* stream) {
+  TS_API_BEGIN(e)
+  SampleCtl ctl;
+  ctl.temperature = temperature; ctl.top_k = top_k; ctl.logp_out = logp_out;
+  check_sample_ctl(ctl, noise);
+  body_generate(e, mfcc, label, noise, codes, poses, B, M, stream, &ctl);
   TS_API_END(e)
 }

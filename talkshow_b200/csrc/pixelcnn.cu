@@ -465,6 +465,10 @@ struct PixArgs {
   int B, T0, Ttot, log_r0, L, nstages, ncta, fused;
   unsigned long long* trace;   // [nstages][ncta][4] globaltimer stamps of row trace_row (debug builds of the kernel only)
   int trace_row;
+  // sampling controls, read by the WARP instantiations only (kept last: the fields above keep their offsets)
+  float temperature;
+  int top_k;
+  float* logp_out;     // [B][Ttot-T0][2] or null
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -975,11 +979,205 @@ __device__ void run_matmul_task(const PixTask& t, const PixArgs& A, int r, const
   }
 }
 
+// ---- sampling controls (WARP instantiations): temperature, top-k, greedy, log-likelihood of the draw -----------------
+// 256 threads own the 2048 logits of one draw, thread tid codes tid + 256 j; `Bar` synchronises those threads.
+struct CtaBar { __device__ __forceinline__ void operator()() const { __syncthreads(); } };
+
+// order-preserving uint32 key of a logit; -0 is folded onto +0 so that keys compare like the floats
+__device__ __forceinline__ uint32_t logit_key(float x) {
+  const uint32_t u = __float_as_uint(x == 0.f ? 0.f : x);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+template <class Bar>
+__device__ __forceinline__ float cta_max8(float v, float* sf, Bar bar) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  if (lane == 0) sf[warp] = v;
+  bar();
+  v = sf[0];
+#pragma unroll
+  for (int w = 1; w < 8; ++w) v = fmaxf(v, sf[w]);
+  bar();
+  return v;
+}
+// same summation order as the default sampler's softmax denominator
+template <class Bar>
+__device__ __forceinline__ float cta_sum8(float v, float* sf, Bar bar) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if (lane == 0) sf[warp] = v;
+  bar();
+  v = sf[0];
+#pragma unroll
+  for (int w = 1; w < 8; ++w) v += sf[w];
+  bar();
+  return v;
+}
+
+// Key of the k-th largest of the 2048 logits, multiplicity counted (1 <= k <= 2048): a 4-pass radix select over 8-bit
+// digits, most significant first, on integer shared-memory histograms (deterministic: no float atomics, the result
+// does not depend on the order of the increments).  hist: 256 words, sel: 2 words.
+template <class Bar>
+__device__ __forceinline__ uint32_t kth_largest_key(const uint32_t (&key)[8], int k, unsigned* hist, unsigned* sel, Bar bar) {
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  uint32_t prefix = 0u, pmask = 0u;
+  unsigned krem = (unsigned)k;   // rank still to find among the keys that match `prefix` (always <= their count)
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    hist[tid] = 0u;
+    bar();
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      if ((key[j] & pmask) == prefix) atomicAdd(&hist[(key[j] >> shift) & 255u], 1u);
+    bar();
+    if (warp == 0) {
+      // lane owns digits 255 - 8 lane - i, i = 0..7 (descending): the digit where the count from the top reaches krem
+      unsigned c[8], s = 0u;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) { c[i] = hist[255 - 8 * lane - i]; s += c[i]; }
+      unsigned incl = s;
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned v = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += v;
+      }
+      unsigned before = incl - s;
+      if (before < krem && krem <= incl) {
+        bool found = false;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          if (!found && before + c[i] >= krem) { sel[0] = 255u - 8u * lane - i; sel[1] = krem - before; found = true; }
+          before += c[i];
+        }
+      }
+    }
+    bar();
+    prefix |= sel[0] << shift;
+    pmask |= 255u << shift;
+    krem = sel[1];
+  }
+  return prefix;
+}
+
+// Block-wide (value, index) maximum with first-index ties, same combine order as the default draw; every thread gets the
+// index (0x7fffffff when no thread had a candidate).
+template <class Bar>
+__device__ __forceinline__ long long cta_argmax(float bv, int bi, float* sf, int* si, long long* scode, Bar bar) {
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+  }
+  if (lane == 0) { sf[warp] = bv; si[warp] = bi; }
+  bar();
+  if (tid == 0) {
+    for (int w = 1; w < 8; ++w)
+      if (sf[w] > bv || (sf[w] == bv && si[w] < bi)) { bv = sf[w]; bi = si[w]; }
+    *scode = bi;
+  }
+  bar();
+  return *scode;
+}
+
+// first index of the maximum of the 2048 logits (0x7fffffff when every logit is NaN)
+template <class Bar>
+__device__ __forceinline__ long long cta_first_argmax(const float (&l)[8], float* sf, int* si, long long* scode, Bar bar) {
+  float bv = -INFINITY;
+  int bi = 0x7fffffff;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int n = threadIdx.x + 256 * j;
+    if (l[j] > bv || (l[j] == bv && n < bi)) { bv = l[j]; bi = n; }
+  }
+  return cta_argmax(bv, bi, sf, si, scode, bar);
+}
+
+// One controlled draw over the raw logits l (include/talkshow_b200.h, ts_pixelcnn_sample):
+//   temperature 0: first-index argmax of l (q is not read);
+//   else s = l / temperature (IEEE division), codes below the k-th largest logit -> -inf, then the default draw
+//   argmax((exp(s - max s) / sum) / q) with first-index ties, over the kept codes only.
+// At temperature 1 without truncation this is the default sampler's arithmetic step for step (s == l).
+// A temperature so small that max(l) / temperature overflows makes every p / q NaN, so no code wins the draw: the code is
+// then the greedy one, the limit of the tempered draw as the temperature goes to 0.  The returned code always lies in
+// [0, 2048): logits that are all NaN give code 0.
+// logp_dst (may be null) receives (l[code] - max l) - log(sum exp(l - max l)).  scratch: 16 + 256 + 2 words from red.
+template <class Bar>
+__device__ __forceinline__ long long draw_controlled(const float (&l)[8], const float (&q)[8], float temperature, int top_k, float* red,
+                                     float* logp_dst, Bar bar) {
+  const int tid = threadIdx.x;
+  float* sf = red;
+  int* si = reinterpret_cast<int*>(red + 16);
+  long long* scode = reinterpret_cast<long long*>(red + 32);
+  unsigned* hist = reinterpret_cast<unsigned*>(red + 64);
+  unsigned* sel = reinterpret_cast<unsigned*>(red + 320);
+  float mx = l[0];
+#pragma unroll
+  for (int j = 1; j < 8; ++j) mx = fmaxf(mx, l[j]);
+  mx = cta_max8(mx, sf, bar);
+  const bool greedy = temperature == 0.f;
+  const bool truncate = !greedy && top_k > 0 && top_k < PIX_NCODE;
+  bool keep[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) keep[j] = true;
+  if (truncate) {
+    uint32_t key[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) key[j] = logit_key(l[j]);
+    const uint32_t kth = kth_largest_key(key, top_k, hist, sel, bar);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) keep[j] = key[j] >= kth;
+  }
+  float sum_raw = 0.f;
+  long long code;
+  if (greedy) {
+    code = cta_first_argmax(l, sf, si, scode, bar);
+  } else {
+    float bv = -INFINITY;
+    int bi = 0x7fffffff;
+    // max_i (l_i / t) = (max_i l_i) / t: a correctly rounded division by t > 0 is monotone, and the maximum is always kept
+    const float mxs = mx / temperature;
+    float ex[8], sum = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { ex[j] = keep[j] ? expf(l[j] / temperature - mxs) : 0.f; sum += ex[j]; }
+    sum = cta_sum8(sum, sf, bar);
+    if (temperature == 1.f && !truncate) sum_raw = sum;   // s == l: the softmax denominator is the untempered one
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int n = tid + 256 * j;
+      const float v = (ex[j] / sum) / q[j];
+      if (keep[j] && (v > bv || (v == bv && n < bi))) { bv = v; bi = n; }
+    }
+    code = cta_argmax(bv, bi, sf, si, scode, bar);
+    // every p / q NaN (s = l / temperature overflowed): the greedy code.  `code` is the same in every thread, so the
+    // barriers inside the branch are reached by the whole CTA.
+    if (code == 0x7fffffff) code = cta_first_argmax(l, sf, si, scode, bar);
+  }
+  if (code >= PIX_NCODE) code = 0;   // all logits NaN: keep the embedding gather inside the table
+  if (logp_dst) {
+    if (greedy || temperature != 1.f || truncate) {
+      float s = 0.f;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) s += expf(l[j] - mx);
+      sum_raw = cta_sum8(s, sf, bar);
+    }
+    if (tid == (int)(code & 255)) {
+      // l[code >> 8] as a sum of selected terms: a plain select chain is turned into an indexed load of a local copy of l
+      const int jc = (int)(code >> 8);
+      float lc = 0.f;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) lc += j == jc ? l[j] : 0.f;
+      *logp_dst = (lc - mx) - logf(sum_raw);
+    }
+  }
+  return code;
+}
+
 // softmax over 2048 logits + categorical draw = argmax(p / q) (ATen multinomial, num_samples = 1),
 // then embedding gather of the sampled code into the E ring.  One CTA per sample.
 // QPRE (persistent kernel): the sampler noise of this position was loaded before the grid-barrier wait (it is an
 // input of the call, independent of every stage) and arrives in qpre[8].
-template <int MB, bool QPRE = false>
+// WARP: the draw applies the sampling controls of A (draw_controlled); otherwise the default draw below.
+template <int MB, bool QPRE = false, bool WARP = false>
 __device__ void run_sample_task(const PixTask& t, const PixArgs& A, int r, int m, float* red, const float* qpre = nullptr) {
   constexpr int SEG = PIX_D * MB;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -1000,7 +1198,20 @@ __device__ void run_sample_task(const PixTask& t, const PixArgs& A, int r, int m
     }
   }
   long long code;
-  if (!forced) {
+  if constexpr (WARP) {
+    if (!forced) {
+      float qv[8];
+      if (A.temperature > 0.f) {
+        const float* q = A.noise + ((size_t)(2 * (r - A.T0) + c) * A.B + m) * PIX_NCODE;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) qv[j] = QPRE ? qpre[j] : q[tid + 256 * j];
+      }
+      float* lp = A.logp_out ? A.logp_out + ((size_t)m * (A.Ttot - A.T0) + (r - A.T0)) * 2 + c : nullptr;
+      code = draw_controlled(l, qv, A.temperature, A.top_k, red, lp, CtaBar());
+    } else {
+      code = A.pre[((size_t)m * A.T0 + r) * 2 + c];
+    }
+  } else if (!forced) {
     float mx = l[0];
 #pragma unroll
     for (int j = 1; j < 8; ++j) mx = fmaxf(mx, l[j]);
@@ -1073,7 +1284,8 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
 // TRACE: a second instantiation of the persistent kernel that stamps, for one latent row, when each CTA's thread 0
 // has its weights, leaves the grid barrier, finishes its task and has arrived again (ts_pixelcnn_trace): the
 // measurement the stage cost model and the CTA split should be fitted to.  The default kernel is TRACE = false.
-template <bool PERSISTENT, int PIPE, bool TRACE = false, bool S2 = false, int MB = 64>
+// WARP: the sample stage applies the sampling controls of A (ts_pixelcnn_sample); every other stage is unchanged.
+template <bool PERSISTENT, int PIPE, bool TRACE = false, bool S2 = false, int MB = 64, bool WARP = false>
 __global__ void __launch_bounds__(PIX_THREADS, 1) pixelcnn_kernel(PixArgs A, int r_single, int s_single) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float* wbuf = reinterpret_cast<float*>(smem_raw);
@@ -1086,7 +1298,7 @@ __global__ void __launch_bounds__(PIX_THREADS, 1) pixelcnn_kernel(PixArgs A, int
     // debug cross-check mode: one launch per stage, weights copied synchronously
     const PixTask t = A.table[(size_t)s_single * A.ncta + cta];
     if (!task_active(t, r_single, A.log_r0)) return;
-    if (t.epi == EPI_SAMPLE) { if (cta < A.B) run_sample_task<MB>(t, A, r_single, cta, red); return; }
+    if (t.epi == EPI_SAMPLE) { if (cta < A.B) run_sample_task<MB, false, WARP>(t, A, r_single, cta, red); return; }
     const int nf = (t.K + 1) * t.rpad;
     for (int i = tid; i < nf; i += PIX_THREADS) wbuf[i] = A.blob[t.wofs + i];
     __syncthreads();
@@ -1135,7 +1347,7 @@ __global__ void __launch_bounds__(PIX_THREADS, 1) pixelcnn_kernel(PixArgs A, int
     pre.a = pre.b = 0.f; pre.valid = false;
     if (active && t.epi != EPI_SAMPLE) pre = prefetch_epilogue<MB, S2>(t, A, r);   // in flight while we wait below
     float qpre[8];   // the sampler noise of this position is an input of the call: in flight while we wait at the barrier
-    if (active && t.epi == EPI_SAMPLE && cta < A.B && r >= A.T0) {
+    if (active && t.epi == EPI_SAMPLE && cta < A.B && r >= A.T0 && (!WARP || A.temperature > 0.f)) {   // greedy: no noise
       const float* q = A.noise + ((size_t)(2 * (r - A.T0) + t.col) * A.B + cta) * PIX_NCODE;
 #pragma unroll
       for (int j = 0; j < 8; ++j) qpre[j] = __ldcs(q + tid + 256 * j);
@@ -1149,7 +1361,7 @@ __global__ void __launch_bounds__(PIX_THREADS, 1) pixelcnn_kernel(PixArgs A, int
     if constexpr (TRACE) { if (tr) tr[1] = globaltimer_ns(); }
     if (active) {
       if (t.epi == EPI_SAMPLE) {
-        if (cta < A.B) run_sample_task<MB, true>(t, A, r, cta, red, qpre);
+        if (cta < A.B) run_sample_task<MB, true, WARP>(t, A, r, cta, red, qpre);
       }
       else run_matmul_task<PIPE, MB, S2>(t, A, r, wbuf + buf * PIX_WBUF, red, pre);
     }
@@ -1207,7 +1419,7 @@ __global__ void logits_to_ref_kernel(const float* __restrict__ in, float* __rest
 
 static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t* label, const float* noise, int noise_B,
                            int64_t* idx_out, float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s,
-                           bool logits_all) {
+                           bool logits_all, const SampleCtl* ctl) {
   PixelPlan* P = e->pix;
   Plan3* Q = (Plan3*)P->p3;
   const int Ttot = T0 + T, D = P->D;
@@ -1234,7 +1446,7 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
   (void)noise_B;
 
   if (v3) {   // cluster-resident executor (pixelcnn3.inc): any batch size, clusters of 16 CTAs per 4 / 8 samples
-    launch_pixelcnn3(e, P, Q, audv, audh, label, noise, idx_out, logits_out, B, T0, Ttot, pre, logits_all, arena3, MB3, s);
+    launch_pixelcnn3(e, P, Q, audv, audh, label, noise, idx_out, logits_out, B, T0, Ttot, pre, logits_all, arena3, MB3, s, ctl);
     return;
   }
   if (B > PIX_MB)
@@ -1262,6 +1474,8 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
   A.B = B; A.T0 = T0; A.Ttot = Ttot; A.log_r0 = logits_all ? 0 : T0; A.L = P->L; A.nstages = P->nstages; A.ncta = P->ncta;
   A.fused = P->fused ? 1 : 0;
   A.trace = P->d_trace; A.trace_row = P->trace_row;
+  const SampleCtl c = ctl ? *ctl : SampleCtl();
+  A.temperature = c.temperature; A.top_k = c.top_k; A.logp_out = c.logp_out;
   if (e->pixel_mode == 0) {
     // A/B switch: 0 = burst loads + scalar FFMA, 4 = pipelined loads + scalar FFMA, 5 (default) = pipelined loads + paired FMAs (fma2)
     static const int pipe = getenv("TS_PIX_PIPE") ? atoi(getenv("TS_PIX_PIPE")) : 5;
@@ -1271,6 +1485,13 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
     if (MB == 8) fn = (void*)pixelcnn_kernel<true, 5, false, false, 8>;
     if (tracing) fn = MB == 16 ? (void*)pixelcnn_kernel<true, 5, true, false, 16> : (void*)pixelcnn_kernel<true, 5, true>;
     if (P->sched == 2) fn = tracing ? (void*)pixelcnn_kernel<true, 5, true, true> : (void*)pixelcnn_kernel<true, 5, false, true>;
+    if (ctl) {   // sampling controls: the WARP instantiation of the default pipeline (no stage-trace variant)
+      fn = MB == 8 ? (void*)pixelcnn_kernel<true, 5, false, false, 8, true>
+           : MB == 16 ? (void*)pixelcnn_kernel<true, 5, false, false, 16, true>
+           : MB == 32 ? (void*)pixelcnn_kernel<true, 5, false, false, 32, true>
+           : P->sched == 2 ? (void*)pixelcnn_kernel<true, 5, false, true, 64, true>
+                           : (void*)pixelcnn_kernel<true, 5, false, false, 64, true>;
+    }
     TS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PIX_SMEM));
     int rs = 0, ss = 0;
     void* args[] = {&A, &rs, &ss};
@@ -1301,6 +1522,13 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
     if (MB == 32) fn1 = pixelcnn_kernel<false, 0, false, false, 32>;
     if (MB == 16) fn1 = pixelcnn_kernel<false, 0, false, false, 16>;
     if (MB == 8) fn1 = pixelcnn_kernel<false, 0, false, false, 8>;
+    if (ctl) {
+      fn1 = MB == 8 ? pixelcnn_kernel<false, 0, false, false, 8, true>
+            : MB == 16 ? pixelcnn_kernel<false, 0, false, false, 16, true>
+            : MB == 32 ? pixelcnn_kernel<false, 0, false, false, 32, true>
+            : P->sched == 2 ? pixelcnn_kernel<false, 0, false, true, 64, true>
+                            : pixelcnn_kernel<false, 0, false, false, 64, true>;
+    }
     TS_CUDA(cudaFuncSetAttribute(fn1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PIX_SMEM));
     for (int r = 0; r < Ttot; ++r)
       for (int st = 0; st < P->nstages; ++st) {
@@ -1320,9 +1548,17 @@ void pixel_destroy(ts_engine* e) {
 }
 
 void pixelcnn_generate_act(ts_engine* e, const Act3& aud, const int64_t* label, const float* noise, int64_t* idx_out,
-                           float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s, bool logits_all) {
+                           float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s, bool logits_all,
+                           const SampleCtl* ctl) {
   if (!e->pix) fail(TS_ERR_NOT_LOADED, "pixelcnn weights not loaded");
-  generate_chunk(e, aud, 0, label, noise, B, idx_out, logits_out, B, T, pre, T0, s, logits_all);
+  generate_chunk(e, aud, 0, label, noise, B, idx_out, logits_out, B, T, pre, T0, s, logits_all, ctl);
+}
+
+void check_sample_ctl(const SampleCtl& c, const float* noise) {
+  if (!std::isfinite(c.temperature) || c.temperature < 0.f)
+    fail(TS_ERR_INVALID, "pixelcnn sample: temperature %g (must be finite and >= 0)", (double)c.temperature);
+  if (c.top_k < 0 || c.top_k > PIX_NCODE) fail(TS_ERR_INVALID, "pixelcnn sample: top_k %d outside [0, %d]", c.top_k, PIX_NCODE);
+  if (c.temperature > 0.f && !noise) fail(TS_ERR_INVALID, "pixelcnn sample: noise is NULL with temperature %g > 0", (double)c.temperature);
 }
 
 }  // namespace ts
@@ -1452,22 +1688,40 @@ static void check_pix(ts_engine* e, int B, int T) {
   if (B <= 0 || T <= 0) fail(TS_ERR_INVALID, "pixelcnn: B=%d T=%d", B, T);
 }
 
-extern "C" int ts_pixelcnn_generate(ts_engine* e, const float* aud, const int64_t* label, const float* noise,
-                                    int64_t* idx_out, float* logits_out, int B, int T, const int64_t* pre_latents, int T0,
-                                    void* stream) {
-  TS_API_BEGIN(e)
+// ctl = nullptr: the default sampler (ts_pixelcnn_generate); else the sampling controls of ts_pixelcnn_sample
+static void pixelcnn_generate_call(ts_engine* e, const float* aud, const int64_t* label, const float* noise, int64_t* idx_out,
+                                   float* logits_out, int B, int T, const int64_t* pre_latents, int T0, void* stream,
+                                   const SampleCtl* ctl) {
   check_pix(e, B, T);
   if (T0 < 0 || (T0 > 0 && !pre_latents)) fail(TS_ERR_INVALID, "pixelcnn: T0=%d without pre_latents", T0);
+  if (ctl) check_sample_ctl(*ctl, noise);
   cudaStream_t s = (cudaStream_t)stream;
   auto body = [&] {
     Act3 a = new_act(e, B, T0 + T, 256, 0, s);
     nct_to_act(e, aud, 256, a, s);
-    pixelcnn_generate_act(e, a, label, noise, idx_out, logits_out, B, T, pre_latents, T0, s);
+    pixelcnn_generate_act(e, a, label, noise, idx_out, logits_out, B, T, pre_latents, T0, s, false, ctl);
   };
   e->ws.begin_sizing(); body();
   size_t need = e->ws.need;
   e->ws.buf.ensure(need + 256);
   e->ws.begin(need); body();
+}
+
+extern "C" int ts_pixelcnn_generate(ts_engine* e, const float* aud, const int64_t* label, const float* noise,
+                                    int64_t* idx_out, float* logits_out, int B, int T, const int64_t* pre_latents, int T0,
+                                    void* stream) {
+  TS_API_BEGIN(e)
+  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, nullptr);
+  TS_API_END(e)
+}
+
+extern "C" int ts_pixelcnn_sample(ts_engine* e, const float* aud, const int64_t* label, const float* noise,
+                                  int64_t* idx_out, float* logits_out, int B, int T, const int64_t* pre_latents, int T0,
+                                  float temperature, int top_k, float* logp_out, void* stream) {
+  TS_API_BEGIN(e)
+  SampleCtl ctl;
+  ctl.temperature = temperature; ctl.top_k = top_k; ctl.logp_out = logp_out;
+  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, &ctl);
   TS_API_END(e)
 }
 

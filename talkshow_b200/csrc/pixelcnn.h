@@ -71,10 +71,20 @@ struct PixelPlan {
   int64_t timed_rows = 0, timed_launches = 0;
 };
 
-// aud: AudioEncoder output, channel-last [B, T0+T, 256].
+// Sampling controls of ts_pixelcnn_sample / ts_body_sample (include/talkshow_b200.h).  A call without them runs the
+// default sampler kernels; a call with them runs the WARP instantiations, whose only difference is the draw.
+struct SampleCtl {
+  float temperature = 1.f;   // > 0: softmax(l / temperature); 0: greedy (first-index argmax of l, noise unread)
+  int top_k = 0;             // 0 or 2048: off; else keep codes with l >= the k-th largest logit
+  float* logp_out = nullptr; // [B,T,2] log_softmax(l)[code] of the untempered, untruncated model, or null
+};
+// Validates the controls (TS_ERR_INVALID): temperature finite and >= 0, top_k in [0, 2048], noise given when sampling.
+void check_sample_ctl(const SampleCtl& c, const float* noise);
+
+// aud: AudioEncoder output, channel-last [B, T0+T, 256].  ctl = nullptr: the default sampler.
 void pixelcnn_generate_act(ts_engine* e, const Act3& aud, const int64_t* label, const float* noise, int64_t* idx_out,
                            float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s,
-                           bool logits_all = false);
+                           bool logits_all = false, const SampleCtl* ctl = nullptr);
 // idx [B,T,2] -> idx_c [2][B][T]; optionally copies idx to codes_out
 void split_codes(ts_engine* e, const int64_t* idx, int64_t* idx_c, int B, int T, int64_t* codes_out, cudaStream_t s);
 void pixel_destroy(ts_engine* e);

@@ -7,12 +7,45 @@ CUDA stream of the engine's device and returns without synchronising.
 from __future__ import annotations
 
 import ctypes as C
+import math
 
 import torch
 
 from . import _lib
 
 PIX_TILE = 64  # samples per PixelCNN launch (csrc/pixelcnn.h PIX_MB)
+NCODE = 2048   # codes of the body prior
+
+
+def check_sample_controls(temperature, top_k):
+    """Validate the values of the sampler's controls (ValueError): temperature finite and >= 0 (0 = greedy decoding),
+    top_k an integer in [0, 2048] (0 = off)."""
+    try:
+        t = float(temperature)
+    except (TypeError, ValueError):
+        raise ValueError("temperature must be a number, got %r" % (temperature,))
+    if not math.isfinite(t) or t < 0:
+        raise ValueError("temperature must be finite and >= 0 (0 = greedy), got %r" % (temperature,))
+    if isinstance(top_k, bool) or int(top_k) != top_k or not 0 <= int(top_k) <= NCODE:
+        raise ValueError("top_k must be an integer in [0, %d] (0 = off), got %r" % (NCODE, top_k))
+
+
+def sample_controls(temperature=1.0, top_k=0, keep_logp=False):
+    """Validated keyword arguments of ``Engine.pixelcnn_generate`` / ``body_generate`` for these controls; empty at the
+    defaults, so that those calls keep the default entry points (ts_pixelcnn_generate / ts_body_generate)."""
+    check_sample_controls(temperature, top_k)
+    if float(temperature) == 1.0 and not top_k and not keep_logp:
+        return {}
+    return dict(temperature=temperature, top_k=top_k, want_logp=bool(keep_logp))
+
+
+def _controlled(temperature, top_k, noise, want_logp):
+    """Engine side: validate the controls and the noise; True when the call goes to ts_pixelcnn_sample / ts_body_sample."""
+    check_sample_controls(temperature, top_k)
+    if noise is None and float(temperature) > 0:
+        raise ValueError("sampling at temperature %g needs the noise tensor (only greedy decoding, temperature 0, "
+                         "runs without)" % float(temperature))
+    return bool(sample_controls(temperature, top_k, want_logp))
 
 
 class Engine:
@@ -159,12 +192,19 @@ class Engine:
         self._check(self.L.ts_audio_encode(self.h, _lib.ptr(mfcc), _lib.ptr(out), B, M, self._s()), "ts_audio_encode")
         return out
 
-    def pixelcnn_generate(self, aud, label, noise, T=None, pre_latents=None, want_logits=False):
+    def pixelcnn_generate(self, aud, label, noise, T=None, pre_latents=None, want_logits=False, temperature=1.0, top_k=0,
+                          want_logp=False):
         """GatedPixelCNN.generate: aud [B,256,T0+T], label [B], noise [2T,B,2048] -> codes [B,T,2]
-        (+ logits [2T,B,2048]).  Batches above the 64-sample tile are chunked here."""
+        (+ logits [2T,B,2048]).  Batches above the 64-sample tile are chunked here.
+
+        Sampling controls (ts_pixelcnn_sample): ``temperature`` (0 = greedy, noise may then be None), ``top_k``
+        (0 = off), ``want_logp`` adds logp [B,T,2] = log_softmax(logits)[code] of the untempered model.  The result is
+        codes, followed by logits when ``want_logits`` and logp when ``want_logp``.  The defaults call
+        ts_pixelcnn_generate."""
+        ctl = _controlled(temperature, top_k, noise, want_logp)
         aud = self._dev(aud, torch.float32)
         label = self._dev(label, torch.int64)
-        noise = self._dev(noise, torch.float32)
+        noise = None if noise is None else self._dev(noise, torch.float32)
         B = aud.shape[0]
         T0 = 0 if pre_latents is None else pre_latents.shape[1]
         T = aud.shape[2] - T0 if T is None else T
@@ -173,24 +213,32 @@ class Engine:
         pre = None if pre_latents is None else self._dev(pre_latents, torch.int64)
         codes = torch.empty(B, T, 2, dtype=torch.int64, device=self.device)
         logits = torch.empty(2 * T, B, 2048, device=self.device) if want_logits else None
+        logp = torch.empty(B, T, 2, device=self.device) if want_logp else None
         aud_c = aud.shape[1]
         assert aud_c == 256, "AudioEncoder output has 256 channels"
         for b0 in range(0, B, PIX_TILE):
             b1 = min(B, b0 + PIX_TILE)
             nb = b1 - b0
             full = nb == B
-            nz = noise if full else noise[:, b0:b1].contiguous()
+            nz = noise if (full or noise is None) else noise[:, b0:b1].contiguous()
             cz = codes if full else torch.empty(nb, T, 2, dtype=torch.int64, device=self.device)
             lz = logits if (full or logits is None) else torch.empty(2 * T, nb, 2048, device=self.device)
-            self._check(self.L.ts_pixelcnn_generate(
-                self.h, _lib.ptr(aud[b0:b1].contiguous()), _lib.ptr(label[b0:b1].contiguous()), _lib.ptr(nz),
-                _lib.ptr(cz), _lib.ptr(lz), nb, T, _lib.ptr(None if pre is None else pre[b0:b1].contiguous()), T0,
-                self._s()), "ts_pixelcnn_generate")
+            pz = logp if (full or logp is None) else torch.empty(nb, T, 2, device=self.device)
+            args = (self.h, _lib.ptr(aud[b0:b1].contiguous()), _lib.ptr(label[b0:b1].contiguous()), _lib.ptr(nz),
+                    _lib.ptr(cz), _lib.ptr(lz), nb, T, _lib.ptr(None if pre is None else pre[b0:b1].contiguous()), T0)
+            if ctl:
+                self._check(self.L.ts_pixelcnn_sample(*args, float(temperature), int(top_k), _lib.ptr(pz), self._s()),
+                            "ts_pixelcnn_sample")
+            else:
+                self._check(self.L.ts_pixelcnn_generate(*args, self._s()), "ts_pixelcnn_generate")
             if not full:
                 codes[b0:b1] = cz
                 if logits is not None:
                     logits[:, b0:b1] = lz
-        return (codes, logits) if want_logits else codes
+                if logp is not None:
+                    logp[b0:b1] = pz
+        out = (codes,) + ((logits,) if want_logits else ()) + ((logp,) if want_logp else ())
+        return out if len(out) > 1 else codes
 
     def pixelcnn_logits(self, aud, label, codes):
         """GatedPixelCNN.forward (teacher forced): -> logits [B,2048,T,2]."""
@@ -313,26 +361,33 @@ class Engine:
                                            self._s()), "ts_face_forward")
         return out
 
-    def body_generate(self, mfcc, label, noise, want_codes=True):
-        """fused s2g_body_pixel core: mfcc [B,64,M] -> (codes [B,T,2], poses [B,4T,C]), C = 129 (258 for 6-D)."""
+    def body_generate(self, mfcc, label, noise, want_codes=True, temperature=1.0, top_k=0, want_logp=False):
+        """fused s2g_body_pixel core: mfcc [B,64,M] -> (codes [B,T,2], poses [B,4T,C]), C = 129 (258 for 6-D).
+        Sampling controls as in ``pixelcnn_generate`` (ts_body_sample); ``want_logp`` appends logp [B,T,2]."""
+        ctl = _controlled(temperature, top_k, noise, want_logp)
         mfcc = self._dev(mfcc, torch.float32)
         label = self._dev(label, torch.int64)
-        noise = self._dev(noise, torch.float32)
+        noise = None if noise is None else self._dev(noise, torch.float32)
         B, _, M = mfcc.shape
         if label.numel() == 1 and B > 1:
             label = label.expand(B).contiguous()
         T = self.latent_rows(M)
         codes = torch.empty(B, T, 2, dtype=torch.int64, device=self.device) if want_codes else None
         poses = torch.empty(B, 4 * T, self.vq_dim(0) + self.vq_dim(1), device=self.device)
+        logp = torch.empty(B, T, 2, device=self.device) if want_logp else None
         for b0 in range(0, B, PIX_TILE):
             b1 = min(B, b0 + PIX_TILE)
             full = (b1 - b0) == B
-            nz = noise if full else noise[:, b0:b1].contiguous()
-            self._check(self.L.ts_body_generate(
-                self.h, _lib.ptr(mfcc[b0:b1]), _lib.ptr(label[b0:b1]), _lib.ptr(nz),
-                _lib.ptr(None if codes is None else codes[b0:b1]), _lib.ptr(poses[b0:b1]), b1 - b0, M, self._s()),
-                "ts_body_generate")
-        return codes, poses
+            nz = noise if (full or noise is None) else noise[:, b0:b1].contiguous()
+            args = (self.h, _lib.ptr(mfcc[b0:b1]), _lib.ptr(label[b0:b1]), _lib.ptr(nz),
+                    _lib.ptr(None if codes is None else codes[b0:b1]), _lib.ptr(poses[b0:b1]), b1 - b0, M)
+            if ctl:
+                self._check(self.L.ts_body_sample(*args, float(temperature), int(top_k),
+                                                  _lib.ptr(None if logp is None else logp[b0:b1]), self._s()),
+                            "ts_body_sample")
+            else:
+                self._check(self.L.ts_body_generate(*args, self._s()), "ts_body_generate")
+        return (codes, poses, logp) if want_logp else (codes, poses)
 
     # -- the single collective of the path, inside the library (ts_allgather over a dlopen'ed NCCL) ----------------
     @staticmethod

@@ -10,6 +10,7 @@ import torch
 
 from ..data_utils.lower_body import c_index_3d, c_index_6d
 from ..data_utils.utils import get_mfcc_sepa, get_mfcc_ta, load_wav
+from ..engine import check_sample_controls, sample_controls
 from .base import draw_sampler_noise, resolve_device, shared_engine, strip_module
 
 
@@ -109,8 +110,9 @@ class TrainWrapper:
                        continuity=False, id=None, fps=15, sr=22000, B=1, am=None, am_sr=None, frame=0, **kwargs):
         """(aud_fn) -> generated motion, numpy (B, F, 129).  Reference: :232-289."""
         assert self.args.infer, "train mode"
+        ctl = {k: kwargs[k] for k in ("temperature", "top_k", "keep_logp") if k in kwargs}
         if continuity:
-            return self._infer_continuity(aud_fn, id, fps, sr, B)
+            return self._infer_continuity(aud_fn, id, fps, sr, B, **ctl)
         if torch.is_tensor(aud_fn) or isinstance(aud_fn, np.ndarray):
             aud_feat = np.asarray(aud_fn, dtype=np.float32)          # already (M, 64) features
             mfcc = torch.from_numpy(np.ascontiguousarray(aud_feat.T))[None].repeat(B, 1, 1)   # [B,64,M]
@@ -121,40 +123,58 @@ class TrainWrapper:
             aud_feat = get_mfcc_ta(aud_fn, sr=sr, fps=fps, smlpx=True, type="mfcc", am=am)
             mfcc = torch.from_numpy(np.ascontiguousarray(aud_feat.T))[None].repeat(B, 1, 1)
         label = torch.tensor([0]) if id is None else id.reshape(-1).repeat(B)[:B] if id.numel() == 1 else id
-        return self.generate(mfcc, label, noise_fn=kwargs.get("noise_fn")).cpu().numpy()
+        return self.generate(mfcc, label, noise_fn=kwargs.get("noise_fn"), **ctl).cpu().numpy()
 
-    def generate(self, aud, id, frame_num=0, noise_fn=None):
+    def generate(self, aud, id, frame_num=0, noise_fn=None, temperature=1.0, top_k=0, keep_logp=False):
         """tensor API (:306-326): aud [B,64,M] features, id [B] -> torch (B, F, 129) on the device.
         (The reference's version passes decode()'s tuple to torch.cat and raises; this returns the
-        tensor its infer_on_audio builds.)"""
+        tensor its infer_on_audio builds.)
+
+        Sampling controls of the prior (Engine.pixelcnn_generate): ``temperature`` (0 = greedy decoding, which draws no
+        noise), ``top_k`` (0 = off); ``keep_logp`` keeps each draw's log-likelihood under the untempered prior as
+        self.last_logp [B,T,2].  The defaults draw exactly like the reference."""
         mfcc = aud.to(torch.float32)
         B, _, M = mfcc.shape
         T = self.engine.latent_rows(M)
-        noise = self._noise(T, B) if noise_fn is None else noise_fn(T, B)      # [2T,B,2048] Exp(1) draws (RNG contract)
-        codes, poses = self.engine.body_generate(mfcc, id.to(torch.int64), noise)
-        self.last_codes = codes
+        noise = self._draw_noise(T, B, noise_fn, temperature, top_k)
+        out = self.engine.body_generate(mfcc, id.to(torch.int64), noise, **sample_controls(temperature, top_k, keep_logp))
+        self.last_codes, poses = out[0], out[1]
+        self.last_logp = out[2] if keep_logp else None
         return poses
 
-    def infer(self, aud_feat, frame, id, B, pre_latents=None, pre_audio=None, pre_pose=None):
+    def _draw_noise(self, T, B, noise_fn, temperature, top_k):
+        """[2T,B,2048] Exp(1) draws (RNG contract), or None for greedy decoding (controls validated first)."""
+        check_sample_controls(temperature, top_k)
+        if float(temperature) == 0:
+            return None
+        return self._noise(T, B) if noise_fn is None else noise_fn(T, B)
+
+    def infer(self, aud_feat, frame, id, B, pre_latents=None, pre_audio=None, pre_pose=None, noise_fn=None,
+              temperature=1.0, top_k=0, keep_logp=False):
         """The reference's inner call (:291-304): aud_feat [B,M,64] (time-major features of ONE chunk) ->
         (latents [B,T,2], audio [B,256,T,2], body [B,39,4T], hand [B,90,4T]).  ``pre_latents`` / ``pre_audio`` (the first
         two results of the previous chunk's call) condition the sampler on that chunk (GatedPixelCNN.generate :158-165);
         ``pre_pose`` is accepted and unused like in the reference, whose Decoder.forward ignores ``pre_state``
-        (nets/spg/vqvae_1d.py:139-149) — each chunk is decoded on its own."""
+        (nets/spg/vqvae_1d.py:139-149) — each chunk is decoded on its own.  Sampling controls as in ``generate``; with
+        ``keep_logp`` the chunk's logp [B,T,2] is kept as self.last_logp."""
         a = self.engine.audio_encode(aud_feat.transpose(1, 2).contiguous())            # [B,256,T]
         T = a.shape[2]
         label = id.reshape(-1)
+        noise = self._draw_noise(T, B, noise_fn, temperature, top_k)
+        ctl = sample_controls(temperature, top_k, keep_logp)
         if pre_latents is None:
-            latents = self.engine.pixelcnn_generate(a, label, self._noise(T, B))
+            out = self.engine.pixelcnn_generate(a, label, noise, **ctl)
         else:
             pa = pre_audio[..., 0] if pre_audio.dim() == 4 else pre_audio              # [B,256,T0]
-            latents = self.engine.pixelcnn_generate(torch.cat([pa.to(a.device), a], 2), label, self._noise(T, B), T=T,
-                                                    pre_latents=pre_latents)
+            out = self.engine.pixelcnn_generate(torch.cat([pa.to(a.device), a], 2), label, noise, T=T,
+                                                pre_latents=pre_latents, **ctl)
+        latents = out[0] if keep_logp else out
+        self.last_logp = out[1] if keep_logp else None
         body = self.engine.vq_decode(0, latents[..., 0].contiguous())
         hand = self.engine.vq_decode(1, latents[..., 1].contiguous())
         return latents, a.unsqueeze(-1).repeat(1, 1, 1, 2), body, hand
 
-    def _infer_continuity(self, aud_fn, id, fps, sr, B):
+    def _infer_continuity(self, aud_fn, id, fps, sr, B, keep_logp=False, **ctl):
         """continuity=True (:244-269): a 2 s prefix, then the rest conditioned on the prefix's latents and audio.  The two
         chunks go through the audio encoder separately and are DECODED separately, so each chunk sees zero padding at the
         2 s seam."""
@@ -162,9 +182,11 @@ class TrainWrapper:
         feat = torch.from_numpy(np.ascontiguousarray(np.asarray(aud_feat, dtype=np.float32)))[None].repeat(B, 1, 1)   # [B,M,64]
         label = torch.tensor([0]) if id is None else id.reshape(-1).repeat(B)
         pre_pose = {"b": None, "h": None}
-        lat0, audio0, body_0, hand_0 = self.infer(feat[:, :gap], 0, label, B, pre_pose=pre_pose)
+        lat0, audio0, body_0, hand_0 = self.infer(feat[:, :gap], 0, label, B, pre_pose=pre_pose, keep_logp=keep_logp, **ctl)
+        logp0 = self.last_logp
         pre_pose["b"], pre_pose["h"] = body_0[:, :, -4:].transpose(1, 2), hand_0[:, :, -4:].transpose(1, 2)
-        lat1, _, body_1, hand_1 = self.infer(feat[:, gap:], 0, label, B, lat0, audio0, pre_pose)
+        lat1, _, body_1, hand_1 = self.infer(feat[:, gap:], 0, label, B, lat0, audio0, pre_pose, keep_logp=keep_logp, **ctl)
         self.last_codes = torch.cat([lat0, lat1], 1)
+        self.last_logp = torch.cat([logp0, self.last_logp], 1) if keep_logp else None
         body, hand = torch.cat([body_0, body_1], 2), torch.cat([hand_0, hand_1], 2)
         return torch.cat([body, hand], 1).transpose(1, 2).cpu().numpy()
