@@ -223,10 +223,35 @@ double ts_pixelcnn_last_ms(ts_engine* e);
 /* Export the PixelCNN execution plan (stage table + packed weight blob) to host buffers so a test
  * can interpret it on the CPU; sizes are returned when the buffers are NULL. */
 int ts_debug_pixelcnn_plan(ts_engine* e, int32_t* table, int64_t* table_len, float* blob, int64_t* blob_len);
-/* dense C[M,N] = act(A[M,K] W[N,K]^T + bias) through one of the two GEMM kernels (unit tests):
- * mode 0 = fp32 FFMA kernel, 1 = wgmma 3xTF32 kernel (K % 32 == 0), 3 = wgmma fp16-split kernel (K % 64 == 0). */
-int ts_debug_gemm(ts_engine* e, int mode, const float* A, const float* W, const float* bias, float* C, int M, int N,
-                  int K, int act, void* stream);
+/* One Conv1d layer through one dense kernel, built as the nets build it (unit tests): production activation layouts and
+ * operand splits (including the per-layer fp16 weight scale), and no fall-back between kernels.
+ *   y(b, t * y_tmul + y_toff, coff + n) = act( sum_{c, j} W[n][c][j] x(b, t * stride + j - pd, c) + bias[n] + res(b, t, n) )
+ * for t < T_out.  x [B,T,C] and res [B,T_out,N] (or NULL) are device fp32; W_host [N,C,k] (torch Conv1d layout) and
+ * bias_host [N] (or NULL) are host fp32.  x is staged in an activation with x_pad zero rows before and after every item
+ * and x_tail rows after those (filled with NaN in every plane: no conv reads them), res in one with res_pad zero rows.
+ * y, y_plane_hi and y_plane_lo are the whole padded output [B, 2 y_pad + y_T, y_C]: their contents are copied in before
+ * the conv and copied back after it, so rows and columns the conv must not write keep what the caller put there.
+ *   mode 0 FFMA gemm_kernel, 1 wgmma 3xTF32, 6 wgmma fp16-split (the numbering of ts_set_tensor_cores);
+ *   y_split: the output is also stored split in the mode's format -- modes 0 / 1: fp32 hi / lo planes (y unused, may be
+ *     NULL), mode 6: fp16 planes (uint16) beside the full fp32 value in y;
+ *   res_split: the residual is stored split in the mode's format;
+ *   planes_only (mode 6): bit 0 the input, bit 1 the output has fp16 planes only, no fp32 copy (y unused);
+ *   chunk: wgmma k-blocks accumulated before each round-to-nearest add (0 = production, K = 256).
+ * Returns TS_ERR_INVALID, before any launch, for a geometry the mode's kernel does not run (modes 1 / 6: C a multiple of
+ * the k-block of 32 / 64 values, rows per item and x_pad - pd multiples of the stride, y_C and coff multiples of 4).
+ * The engine's ts_set_tensor_cores setting is unchanged afterwards. */
+typedef struct ts_debug_conv {
+  int32_t mode;
+  int32_t B, T, C, x_pad, x_tail;
+  int32_t N, k, stride, pd, T_out, act;  /* act: 0 none, 1 ReLU, 2 LeakyReLU(0.2), 3 GELU (erf) */
+  int32_t y_T, y_C, y_pad, y_tmul, y_toff, coff;
+  int32_t y_split;
+  int32_t res_pad, res_split;
+  int32_t chunk;
+  int32_t planes_only;
+} ts_debug_conv;
+int ts_debug_conv1d(ts_engine* e, const ts_debug_conv* a, const float* x, const float* W_host, const float* bias_host,
+                    const float* res, float* y, void* y_plane_hi, void* y_plane_lo, void* stream);
 /* Dense-contraction kernel for the face network and the VQ decoder (csrc/gemm_tc.cu):
  *   6 (default) Hopper wgmma kernel (128x128 tile) on two-term fp16-split operands (three products per MAC: fp32-grade
  *       results at twice the tf32 rate; operands must stay below 65504 in magnitude -- weights are pre-scaled per layer),

@@ -83,8 +83,8 @@ SYMBOLS = {
     "ts_set_pixelcnn_ctas": (C.c_int, [C.c_void_p, C.c_int]),
     "ts_set_vq_parallel": (C.c_int, [C.c_void_p, C.c_int]),
     "ts_set_tensor_cores": (C.c_int, [C.c_void_p, C.c_int]),
-    "ts_debug_gemm": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
-                                C.c_int, C.c_int, C.c_void_p]),
+    "ts_debug_conv1d": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                  C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 

@@ -1146,12 +1146,7 @@ __global__ void __launch_bounds__(PC_WARPS * 32, 1) posconv_mma_kernel(Act3 x, c
 static unsigned short* pack_posconv16(ts_engine* e, const float* w, float* unscale) {
   float mx = 0.f;
   for (size_t i = 0; i < (size_t)768 * 48 * 128; ++i) mx = std::max(mx, std::fabs(w[i]));
-  int shift = 0;
-  if (mx > 0.f && std::isfinite(mx)) {
-    int ex;
-    std::frexp(mx, &ex);
-    shift = std::min(14, std::max(0, 14 - ex));
-  }
+  const int shift = split16_shift(mx);
   const float sc = std::ldexp(1.0f, shift);
   *unscale = std::ldexp(1.0f, -shift);
   std::vector<unsigned short> P((size_t)16 * 128 * 2 * 48 * PC_LD, 0);

@@ -16,14 +16,17 @@
 // Two operand formats, one kernel:
 //  * fp16 split (ts_set_tensor_cores(e, 6), the default): h = fp16(x), l = fp16(x - h) — 11 + 11 significant bits, the
 //    same as two tf32 terms — products as wgmma f16 (k16), which runs at twice the tf32 rate: a 128-byte k-block holds 64 K
-//    values instead of 32.  Range: |x| < 65504 (fp16); weights are pre-scaled by a power of two per layer so their low
-//    plane stays normal (undone exactly in the epilogue); activations whose low plane underflows lose absolute accuracy
-//    below 2^-25 only.
+//    values instead of 32.  Range: |x| < 65504 (fp16); the weights of every layer are pre-scaled by the power of two
+//    (split16_shift) that puts max|W| in [2^13, 2^14) whatever the layer's magnitude -- the high plane cannot overflow and
+//    the low plane stays normal for every weight within about 2^-16 of max|W| -- and the epilogue undoes it exactly;
+//    activations whose low plane underflows lose absolute accuracy below 2^-25 only.
 //  * 3xTF32 (modes 1 / 3 / 4): hi = fp32 with the 13 low mantissa bits cleared, lo = x - hi (exact), wgmma tf32 (k8).
 #include <cuda.h>
 #include <cuda_fp16.h>
 
-#include "kernels.h"
+#include <climits>
+
+#include "convstack.h"
 
 namespace ts {
 
@@ -341,19 +344,17 @@ void split_hi_lo(ts_engine* e, const float* x, float* hi, float* lo, long n, cud
   e->launches++;
   TS_CUDA(cudaGetLastError());
 }
-__global__ void split16_kernel(const float* __restrict__ x, unsigned short* __restrict__ h, unsigned short* __restrict__ l, long n, float scale) {
-  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) split16(x[i] * scale, h[i], l[i]);
+int split16_shift(float max_abs) {
+  if (!(max_abs > 0.f) || !std::isfinite(max_abs)) return 0;   // all-zero (or non-finite) layer: unscaled
+  int ex;
+  std::frexp(max_abs, &ex);                                       // max_abs = m * 2^ex, m in [0.5, 1)
+  return std::min(100, std::max(-100, 14 - ex));                  // 2^+-100 stays a normal float
 }
-// fp16 planes of W * 2^shift; the shift puts max|W| just below 2^14 (clamped to [0, 14]) and comes back as 2^-shift
+// fp16 planes of W * 2^shift (split16_shift); returns the epilogue's 2^-shift
 static float split16_host(const std::vector<float>& w, std::vector<unsigned short>* h, std::vector<unsigned short>* l) {
   float mx = 0.f;
   for (float v : w) mx = std::max(mx, std::fabs(v));
-  int shift = 0;
-  if (mx > 0.f && std::isfinite(mx)) {
-    int ex;
-    std::frexp(mx, &ex);            // mx = m * 2^ex, m in [0.5, 1)
-    shift = std::min(14, std::max(0, 14 - ex));
-  }
+  const int shift = split16_shift(mx);
   const float sc = std::ldexp(1.0f, shift);
   h->resize(w.size());
   l->resize(w.size());
@@ -419,7 +420,7 @@ bool tc_conv_supported(ts_engine* e, const Layer& L, const Act3& x, int stride, 
 
 // y(b, t*y_tmul + y_toff, :) = act( conv(x)(b,t,:) + bias + res(b,t,:) );  x and W must be split (hi/lo)
 void tc_conv1d(ts_engine* e, const Layer& L, const Act3& x, int k, int stride, int pd, const Act3& y, int T_out, int act, const Act3* res,
-               cudaStream_t s, int y_tmul, int y_toff, int coff) {
+               cudaStream_t s, int y_tmul, int y_toff, int coff, int chunk) {
   if (e->ws.sizing) return;
   if (!tc_conv_supported(e, L, x, stride, pd)) fail(TS_ERR_INVALID, "tc_conv1d: unsupported geometry");
   if (!y.p && !y.h16) fail(TS_ERR_INVALID, "tc_conv1d: output without storage");
@@ -443,7 +444,8 @@ void tc_conv1d(ts_engine* e, const Layer& L, const Act3& x, int k, int stride, i
   const void* wl = f16 ? (const void*)L.W_l16 : (const void*)L.W_lo;
   CUtensorMap mBh = make_map(wh, 2, bdims, bstr, bbox, f16), mBl = make_map(wl, 2, bdims, bstr, bbox, f16);
   TcArgs P;
-  P.chunk = 256 / bk;                  // K = 256 per wgmma accumulation chunk
+  if (chunk < 0) fail(TS_ERR_INVALID, "tc_conv1d: chunk %d < 0", chunk);
+  P.chunk = chunk ? chunk : 256 / bk;  // default: K = 256 per wgmma accumulation chunk
   P.oscale = f16 ? L.w_unscale : 1.f;
   P.c_h16 = y.h16 ? y.row_h16(0, y_toff) + coff : nullptr;
   P.c_l16 = y.h16 ? y.row_l16(0, y_toff) + coff : nullptr;
@@ -502,54 +504,123 @@ extern "C" int ts_set_tensor_cores(ts_engine* e, int enable) {
   return TS_OK;
 }
 
-// debug entry: dense C[M,N] = act(A[M,K] W[N,K]^T + bias), mode 0 = FFMA kernel, 1 = wgmma 3xTF32, 3 = wgmma fp16-split
-extern "C" int ts_debug_gemm(ts_engine* e, int mode, const float* A, const float* W, const float* bias, float* C, int M, int N, int K, int act,
-                             void* stream) {
-  TS_API_BEGIN(e)
-  cudaStream_t s = (cudaStream_t)stream;
-  if (mode == 0) {
-    GemmP p;
-    p.A = A; p.W = W; p.bias = bias; p.C = C; p.M = M; p.N = N; p.K = K; p.mper = M; p.a_rs = K; p.kc = K; p.a_ts = K; p.c_rs = N; p.act = act; p.ldw = K;
-    e->ws.sizing = false;
-    launch_gemm(e, p, s);
-  } else if (mode == 3) {
-    if (K % (2 * TC_BK)) fail(TS_ERR_INVALID, "ts_debug_gemm: K must be a multiple of 64 for the fp16-split path");
-    const bool f0 = e->tc_f16;
-    e->tc_f16 = true;
-    e->ws.sizing = false;
-    unsigned short *ah, *al, *wh, *wl;
-    TS_CUDA(cudaMalloc(&ah, (size_t)M * K * 2)); TS_CUDA(cudaMalloc(&al, (size_t)M * K * 2));
-    TS_CUDA(cudaMalloc(&wh, (size_t)N * K * 2)); TS_CUDA(cudaMalloc(&wl, (size_t)N * K * 2));
-    split16_kernel<<<e->sm_count * 8, 256, 0, s>>>(A, ah, al, (long)M * K, 1.f);
-    split16_kernel<<<e->sm_count * 8, 256, 0, s>>>(W, wh, wl, (long)N * K, 256.f);
-    Layer L;
-    L.N = N; L.K = K; L.taps = 1; L.cin = K; L.W_h16 = wh; L.W_l16 = wl; L.w_unscale = 1.f / 256.f; L.bias = const_cast<float*>(bias);
-    Act3 x; x.p = const_cast<float*>(A); x.h16 = ah; x.l16 = al; x.split = true; x.B = 1; x.T = M; x.C = K; x.pad = 0;
-    Act3 y; y.p = C; y.B = 1; y.T = M; y.C = N; y.pad = 0;
-    tc_conv1d(e, L, x, 1, 1, 0, y, M, act, nullptr, s, 1, 0, 0);
-    e->tc_f16 = f0;
-    TS_CUDA(cudaStreamSynchronize(s));
-    cudaFree(ah); cudaFree(al); cudaFree(wh); cudaFree(wl);
-  } else if (mode == 1) {
-    if (K % TC_BK) fail(TS_ERR_INVALID, "ts_debug_gemm: K must be a multiple of 32 for the tensor-core path");
-    const bool f0 = e->tc_f16;
-    e->tc_f16 = false;
-    e->ws.sizing = false;
-    float *ah, *al, *wh, *wl;
-    TS_CUDA(cudaMalloc(&ah, (size_t)M * K * 4)); TS_CUDA(cudaMalloc(&al, (size_t)M * K * 4));
-    TS_CUDA(cudaMalloc(&wh, (size_t)N * K * 4)); TS_CUDA(cudaMalloc(&wl, (size_t)N * K * 4));
-    split_hi_lo(e, A, ah, al, (long)M * K, s);
-    split_hi_lo(e, W, wh, wl, (long)N * K, s);
-    Layer L;
-    L.N = N; L.K = K; L.taps = 1; L.cin = K; L.W_hi = wh; L.W_lo = wl; L.bias = const_cast<float*>(bias);
-    Act3 x; x.p = ah; x.lo = al; x.split = true; x.B = 1; x.T = M; x.C = K; x.pad = 0;
-    Act3 y; y.p = C; y.B = 1; y.T = M; y.C = N; y.pad = 0;
-    tc_conv1d(e, L, x, 1, 1, 0, y, M, act, nullptr, s, 1, 0, 0);
-    e->tc_f16 = f0;
-    TS_CUDA(cudaStreamSynchronize(s));
-    cudaFree(ah); cudaFree(al); cudaFree(wh); cudaFree(wl);
-  } else {
-    fail(TS_ERR_INVALID, "ts_debug_gemm: mode %d (0 = FFMA, 1 = 3xTF32, 3 = fp16-split)", mode);
+namespace ts {
+// x [B, a.T, a.C] -> rows [0, a.T) of every batch item of `a`, in a's storage format (fp32, 3xTF32 pair or fp32 + fp16
+// planes); the tail rows of every plane get NaN: no conv may read them.  Pad rows keep new_act's zeros.
+__global__ void debug_fill_kernel(const float* __restrict__ x, Act3 a) {
+  const int rows = a.T + 2 * a.pad + a.tail;
+  const long n = (long)a.B * rows * a.C;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % a.C), r = (int)((i / a.C) % rows), b = (int)(i / ((long)a.C * rows));
+    const int t = r - a.pad;
+    float v;
+    if (t >= 0 && t < a.T) v = x[((long)b * a.T + t) * a.C + c];
+    else if (r >= a.T + 2 * a.pad) v = __int_as_float(0x7fffffff);
+    else continue;
+    if (a.lo) {
+      const float h = __uint_as_float(__float_as_uint(v) & 0xffffe000u);
+      a.p[i] = h;
+      a.lo[i] = v - h;
+    } else {
+      if (a.p) a.p[i] = v;
+      if (a.h16) split16(v, a.h16[i], a.l16[i]);
+    }
   }
+}
+
+// The engine's dense-kernel switches for one call, restored however the call ends
+struct TcModeGuard {
+  ts_engine* e;
+  bool use_tc, tc_f16;
+  TcModeGuard(ts_engine* e_, int mode) : e(e_), use_tc(e_->use_tc), tc_f16(e_->tc_f16) {
+    e->use_tc = mode != 0;
+    e->tc_f16 = mode == 6;
+  }
+  ~TcModeGuard() {
+    e->use_tc = use_tc;
+    e->tc_f16 = tc_f16;
+  }
+};
+}  // namespace ts
+
+extern "C" int ts_debug_conv1d(ts_engine* e, const ts_debug_conv* a, const float* x, const float* W_host, const float* bias_host,
+                               const float* res, float* y, void* y_plane_hi, void* y_plane_lo, void* stream) {
+  TS_API_BEGIN(e)
+  require_device(e);
+  if (!a || !x || !W_host) fail(TS_ERR_INVALID, "ts_debug_conv1d: a, x and W_host are required");
+  const ts_debug_conv g = *a;
+  const int mode = g.mode;
+  if (mode != 0 && mode != 1 && mode != 6) fail(TS_ERR_INVALID, "ts_debug_conv1d: mode %d (0 = FFMA, 1 = wgmma 3xTF32, 6 = wgmma fp16-split)", mode);
+  if (g.B < 1 || g.T < 1 || g.C < 1 || g.N < 1 || g.k < 1 || g.stride < 1 || g.T_out < 1 || g.x_pad < 0 || g.x_tail < 0 || g.pd < 0 ||
+      g.y_T < 1 || g.y_C < 1 || g.y_pad < 0 || g.y_tmul < 1 || g.y_toff < 0 || g.coff < 0 || g.res_pad < 0 || g.chunk < 0)
+    fail(TS_ERR_INVALID, "ts_debug_conv1d: an empty or negative size");
+  if (g.act < ACT_NONE || g.act > ACT_GELU) fail(TS_ERR_INVALID, "ts_debug_conv1d: act %d (0 none, 1 ReLU, 2 LReLU 0.2, 3 GELU)", g.act);
+  if (g.pd > g.x_pad) fail(TS_ERR_INVALID, "ts_debug_conv1d: conv padding %d > input pad rows %d", g.pd, g.x_pad);
+  if ((long)(g.T_out - 1) * g.stride + g.k > (long)g.T + g.x_pad + g.pd)
+    fail(TS_ERR_INVALID, "ts_debug_conv1d: the window of output %d reaches past the input's back pad rows", g.T_out - 1);
+  if ((long)(g.T_out - 1) * g.y_tmul + g.y_toff >= g.y_T || (long)g.coff + g.N > g.y_C)
+    fail(TS_ERR_INVALID, "ts_debug_conv1d: outputs fall outside y [%d rows, %d columns]", g.y_T, g.y_C);
+  const long rows_in = (long)g.T + 2L * g.x_pad + g.x_tail;
+  if ((long)g.B * rows_in > INT_MAX || (long)g.B * (g.y_T + 2L * g.y_pad) > INT_MAX)
+    fail(TS_ERR_INVALID, "ts_debug_conv1d: more than 2^31 - 1 rows");
+  if (mode == 0) {
+    if (g.C % 4) fail(TS_ERR_INVALID, "ts_debug_conv1d: the FFMA kernel needs C %% 4 == 0 (C = %d)", g.C);
+  } else {
+    const int bk = mode == 6 ? 2 * TC_BK : TC_BK;
+    if (g.C % bk) fail(TS_ERR_INVALID, "ts_debug_conv1d: C %d is not a multiple of the %d-value k-block of mode %d", g.C, bk, mode);
+    if (rows_in % g.stride || (g.x_pad - g.pd) % g.stride)
+      fail(TS_ERR_INVALID, "ts_debug_conv1d: rows per item (%ld) and x_pad - pd (%d) must be multiples of the stride %d", rows_in,
+           g.x_pad - g.pd, g.stride);
+    if (g.y_C % 4 || g.coff % 4)
+      fail(TS_ERR_INVALID, "ts_debug_conv1d: the wgmma epilogue stores 4 columns at a time: y_C %d and coff %d must be multiples of 4", g.y_C,
+           g.coff);
+  }
+  const bool x_planes = (g.planes_only & 1) != 0, y_planes = (g.planes_only & 2) != 0;
+  if (g.planes_only & ~3) fail(TS_ERR_INVALID, "ts_debug_conv1d: planes_only %d (bit 0 input, bit 1 output)", g.planes_only);
+  if ((x_planes || y_planes) && mode != 6) fail(TS_ERR_INVALID, "ts_debug_conv1d: planes-only activations exist in mode 6 only");
+  if (y_planes && !g.y_split) fail(TS_ERR_INVALID, "ts_debug_conv1d: a planes-only output needs y_split");
+  if (g.y_split && (!y_plane_hi || !y_plane_lo)) fail(TS_ERR_INVALID, "ts_debug_conv1d: y_split needs y_plane_hi and y_plane_lo");
+  const bool y_full = !g.y_split || (mode == 6 && !y_planes);   // an fp32 copy of the full value exists
+  if (y_full && !y) fail(TS_ERR_INVALID, "ts_debug_conv1d: y is required");
+
+  // torch Conv1d weight [N][C][k] -> the packed layout [N][k][C] (tap-major), production split
+  std::vector<float> W((size_t)g.N * g.k * g.C);
+  for (int n = 0; n < g.N; ++n)
+    for (int c = 0; c < g.C; ++c)
+      for (int t = 0; t < g.k; ++t) W[((size_t)n * g.k + t) * g.C + c] = W_host[((size_t)n * g.C + c) * g.k + t];
+  LoadScope scope(e, "debug_conv");   // this call's weights replace the previous call's
+  Layer L;
+  L.N = g.N; L.K = g.k * g.C; L.taps = g.k; L.cin = g.C;
+  upload_weights(e, W, &L);
+  if (bias_host) L.bias = e->upload(std::vector<float>(bias_host, bias_host + g.N));
+
+  TcModeGuard guard(e, mode);
+  cudaStream_t s = (cudaStream_t)stream;
+  Act3 xa, ya, ra;
+  run_sized(e, [&] {
+    xa = new_act(e, g.B, g.T, g.C, g.x_pad, s, mode != 0, g.x_tail, x_planes);
+    ya = new_act(e, g.B, g.y_T, g.y_C, g.y_pad, s, g.y_split != 0, 0, y_planes);
+    if (res) ra = new_act(e, g.B, g.T_out, g.N, g.res_pad, s, g.res_split != 0);
+  });
+  auto fill = [&](const float* src, const Act3& dst) {
+    debug_fill_kernel<<<(int)std::min<long>((long)(dst.numel() + 255) / 256, (long)e->sm_count * 16), 256, 0, s>>>(src, dst);
+    e->launches++;
+    TS_CUDA(cudaGetLastError());
+  };
+  fill(x, xa);
+  if (res) fill(res, ra);
+  // y's planes: hi / lo fp32 (modes 0, 1: ya.p is the hi plane) or h16 / l16 (mode 6)
+  const size_t yn = ya.numel();
+  struct Plane { void* dev; void* user; size_t bytes; };
+  const Plane planes[4] = {{ya.p, ya.lo ? y_plane_hi : (void*)y, yn * 4}, {ya.lo, y_plane_lo, yn * 4},
+                           {ya.h16, y_plane_hi, yn * 2}, {ya.l16, y_plane_lo, yn * 2}};
+  for (const Plane& p : planes)
+    if (p.dev) TS_CUDA(cudaMemcpyAsync(p.dev, p.user, p.bytes, cudaMemcpyDeviceToDevice, s));
+  if (mode == 0) conv1d(e, L, xa, g.k, g.stride, g.pd, ya, g.T_out, g.act, res ? &ra : nullptr, s, g.y_tmul, g.y_toff, 0, g.coff);
+  else tc_conv1d(e, L, xa, g.k, g.stride, g.pd, ya, g.T_out, g.act, res ? &ra : nullptr, s, g.y_tmul, g.y_toff, g.coff, g.chunk);
+  for (const Plane& p : planes)
+    if (p.dev) TS_CUDA(cudaMemcpyAsync(p.user, p.dev, p.bytes, cudaMemcpyDeviceToDevice, s));
+  TS_CUDA(cudaStreamSynchronize(s));
+  scope.commit();
   TS_API_END(e)
 }

@@ -82,9 +82,11 @@ void layernorm(ts_engine* e, const Act3& x, const float* g, const float* b, cons
 // ---- tensor-core path (gemm_tc.cu): Hopper wgmma on fp16-split or 3xTF32 operands, TMA-staged ------
 bool tc_conv_supported(ts_engine* e, const Layer& L, const Act3& x, int stride, int pd);
 void tc_conv1d(ts_engine* e, const Layer& L, const Act3& x, int k, int stride, int pd, const Act3& y, int T_out, int act,
-               const Act3* res, cudaStream_t s, int y_tmul = 1, int y_toff = 0, int coff = 0);
+               const Act3* res, cudaStream_t s, int y_tmul = 1, int y_toff = 0, int coff = 0, int chunk = 0);
 void split_hi_lo(ts_engine* e, const float* x, float* hi, float* lo, long n, cudaStream_t s);
 void split_host(const std::vector<float>& w, std::vector<float>* hi, std::vector<float>* lo);
+// power-of-two exponent of a layer's fp16-split weight scale: max|W| * 2^shift lands in [2^13, 2^14) (0 for an all-zero layer)
+int split16_shift(float max_abs);
 // upload W and its (hi, lo) split copies into a Layer
 void upload_weights(ts_engine* e, const std::vector<float>& W, Layer* L);
 // conv through the tensor-core kernel when the geometry allows (and e->use_tc), else the FFMA kernel
