@@ -99,6 +99,43 @@ int ts_pixelcnn_generate(ts_engine* e, const float* aud, const int64_t* label, c
 int ts_pixelcnn_sample(ts_engine* e, const float* aud, const int64_t* label, const float* noise,
                        int64_t* idx_out, float* logits_out, int B, int T, const int64_t* pre_latents, int T0,
                        float temperature, int top_k, float* logp_out, void* stream);
+/* The sampling controls as one struct, with nucleus (top-p) and min-p truncation and the size of each draw's keep set.
+ * The controls apply in the order temperature -> top_k -> top_p -> min_p.  Let l be the 2048 raw logits of one draw and
+ * t = temperature > 0.
+ *  1. keep0 = the top_k set of ts_pixelcnn_sample (on the raw logits, ties kept; every code when off).
+ *  2. e_i = expf(l_i / t - max(l) / t) for the codes of keep0 and 0 for the others, in fp32 (the most likely code has e = 1).
+ *  3. Integer mass w_i = e_i * 2^32 rounded to the nearest integer, ties to even, as uint64; W = sum w_i <= 2^43.  Every
+ *     partial sum of masses is exact in uint64 and in a double, and integer addition is associative: the sums below do not
+ *     depend on the order in which an implementation adds, so the keep set is the same in every executor, batch tile and
+ *     batch.
+ *  4. top_p in (0, 1), 1 = off: with A_i = sum { w_j : l_j > l_i } the mass strictly above code i (-0 compares equal to
+ *     +0), keep i iff (double)A_i < (double)top_p * (double)W, one IEEE double multiplication.  This is the smallest set
+ *     of most likely codes whose mass reaches top_p (TopPLogitsWarper), with the ties at the boundary all kept, like
+ *     top_k.  The most likely code is always kept.
+ *  5. min_p in (0, 1], 0 = off: keep i iff e_i >= min_p (fp32 comparison): probability at least min_p times that of the
+ *     most likely code.  The final keep set is the intersection of 1, 4 and 5.
+ *  6. The draw is that of ts_pixelcnn_sample over the final keep set: argmax((e_i / sum of kept e) / q_i), first-index
+ *     ties, same noise and RNG contract, the same fallback to the greedy code when every e / q is NaN.  A dropped code
+ *     is never drawn.
+ *  7. temperature = 0 (greedy) ignores top_p and min_p as it ignores top_k.  logp_out is the log-softmax of the
+ *     untempered, untruncated logits, as in ts_pixelcnn_sample.
+ *  8. kept_out (may be NULL) [B,T,2] int32, laid out like idx_out: the size of the final keep set of each draw (1 for a
+ *     greedy draw).  Rows forced by pre_latents have no entry.
+ * With top_p = 1 and min_p = 0 the arithmetic is that of ts_pixelcnn_sample step for step. */
+typedef struct ts_sample_ctl {
+  float temperature;   /* as ts_pixelcnn_sample */
+  int32_t top_k;       /* as ts_pixelcnn_sample */
+  float top_p;         /* (0, 1]; 1 = off */
+  float min_p;         /* [0, 1]; 0 = off */
+  float* logp_out;     /* [B,T,2] or NULL */
+  int32_t* kept_out;   /* [B,T,2] or NULL */
+} ts_sample_ctl;
+/* ts_pixelcnn_sample with the controls of ts_sample_ctl; ts_pixelcnn_sample is this call with top_p = 1, min_p = 0 and
+ * kept_out = NULL.  The launches are those of ts_pixelcnn_generate.  TS_ERR_INVALID: ctl NULL, top_p outside (0, 1] or
+ * NaN, min_p outside [0, 1] or NaN, and the conditions of ts_pixelcnn_sample. */
+int ts_pixelcnn_sample_ctl(ts_engine* e, const float* aud, const int64_t* label, const float* noise, int64_t* idx_out,
+                           float* logits_out, int B, int T, const int64_t* pre_latents, int T0,
+                           const ts_sample_ctl* ctl, void* stream);
 /* GatedPixelCNN.forward (teacher forced), :130-150, for rows [0,T): logits_out [B,2048,T,2]. */
 int ts_pixelcnn_logits(ts_engine* e, const float* aud, const int64_t* label, const int64_t* codes,
                        float* logits_out, int B, int T, void* stream);
@@ -162,6 +199,10 @@ int ts_body_generate(ts_engine* e, const float* mfcc, const int64_t* label, cons
  * temperature, top_k, logp_out [B,T,2] (may be NULL); noise may be NULL when temperature = 0. */
 int ts_body_sample(ts_engine* e, const float* mfcc, const int64_t* label, const float* noise, int64_t* codes,
                    float* poses, int B, int M, float temperature, int top_k, float* logp_out, void* stream);
+/* ts_body_generate with the controls of ts_pixelcnn_sample_ctl, same semantics and same error statuses;
+ * ts_body_sample is this call with top_p = 1, min_p = 0 and kept_out = NULL. */
+int ts_body_sample_ctl(ts_engine* e, const float* mfcc, const int64_t* label, const float* noise, int64_t* codes,
+                       float* poses, int B, int M, const ts_sample_ctl* ctl, void* stream);
 
 /* Audio front-end of get_mfcc_ta, data_utils/utils.py:148-177 (SURVEY.md §8f-1): wave [B,N] mono at
  * `sr` Hz -> torchaudio Resample(sr, 22000) -> MFCC(64 coefficients, n_fft 2048, hop 734 = 30 fps, 256 HTK

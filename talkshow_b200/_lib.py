@@ -22,6 +22,11 @@ class ts_tensor(C.Structure):
                 ("shape", C.c_int64 * 6)]
 
 
+class ts_sample_ctl(C.Structure):
+    _fields_ = [("temperature", C.c_float), ("top_k", C.c_int32), ("top_p", C.c_float), ("min_p", C.c_float),
+                ("logp_out", C.c_void_p), ("kept_out", C.c_void_p)]
+
+
 SYMBOLS = {
     "ts_engine_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int]),
     "ts_engine_destroy": (None, [C.c_void_p]),
@@ -46,6 +51,10 @@ SYMBOLS = {
                                      C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_void_p, C.c_void_p]),
     "ts_body_sample": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                  C.c_int, C.c_float, C.c_int, C.c_void_p, C.c_void_p]),
+    "ts_pixelcnn_sample_ctl": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_int, C.c_int, C.c_void_p, C.c_int, C.POINTER(ts_sample_ctl), C.c_void_p]),
+    "ts_body_sample_ctl": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                     C.c_int, C.POINTER(ts_sample_ctl), C.c_void_p]),
     "ts_pixelcnn_logits": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                      C.c_void_p]),
     "ts_pixelcnn_score": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,

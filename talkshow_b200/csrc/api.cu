@@ -303,10 +303,15 @@ extern "C" int ts_body_generate(ts_engine* e, const float* mfcc, const int64_t* 
 
 extern "C" int ts_body_sample(ts_engine* e, const float* mfcc, const int64_t* label, const float* noise, int64_t* codes,
                               float* poses, int B, int M, float temperature, int top_k, float* logp_out, void* stream) {
+  const ts_sample_ctl ctl = {temperature, top_k, 1.f, 0.f, logp_out, nullptr};
+  return ts_body_sample_ctl(e, mfcc, label, noise, codes, poses, B, M, &ctl, stream);
+}
+
+extern "C" int ts_body_sample_ctl(ts_engine* e, const float* mfcc, const int64_t* label, const float* noise, int64_t* codes,
+                                  float* poses, int B, int M, const ts_sample_ctl* ctl, void* stream) {
   TS_API_BEGIN(e)
-  SampleCtl ctl;
-  ctl.temperature = temperature; ctl.top_k = top_k; ctl.logp_out = logp_out;
-  check_sample_ctl(ctl, noise);
-  body_generate(e, mfcc, label, noise, codes, poses, B, M, stream, &ctl);
+  const SampleCtl c = sample_ctl_of(ctl);
+  check_sample_ctl(c, noise);
+  body_generate(e, mfcc, label, noise, codes, poses, B, M, stream, &c);
   TS_API_END(e)
 }

@@ -469,6 +469,8 @@ struct PixArgs {
   float temperature;
   int top_k;
   float* logp_out;     // [B][Ttot-T0][2] or null
+  float top_p, min_p;
+  int* kept_out;       // [B][Ttot-T0][2] or null
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -1058,6 +1060,74 @@ __device__ __forceinline__ uint32_t kth_largest_key(const uint32_t (&key)[8], in
   return prefix;
 }
 
+// Boundary key of nucleus (top-p) sampling over integer masses w (w = 0 for a code that is already dropped; w is
+// non-decreasing in the key): the largest key whose mass strictly above it, A, satisfies (double)A < p * (double)W, W the
+// total mass.  Keeping key >= the result keeps the smallest set of most likely codes whose mass reaches p W, with the
+// ties at the boundary.  The same 4-pass radix select as kth_largest_key, on a histogram of mass instead of counts:
+// integer addition is associative, so neither the histogram nor the result depends on the order of the increments, and
+// every partial sum (<= 2^43) is exact both in uint64 and in a double.  hist: 256 uint64, sel: 1 word.
+template <class Bar>
+__device__ __forceinline__ uint32_t nucleus_key(const uint32_t (&key)[8], const unsigned long long (&w)[8], float p,
+                                                unsigned long long* hist, unsigned* sel, Bar bar) {
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  uint32_t prefix = 0u, pmask = 0u;
+  unsigned long long above = 0ull;   // mass of the keys above every key that matches `prefix` (warp 0 only)
+  double P = 0.0;                    // p W, known once the first pass has the total (warp 0 only)
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    hist[tid] = 0ull;
+    bar();
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      if (w[j] != 0ull && (key[j] & pmask) == prefix) atomicAdd(&hist[(key[j] >> shift) & 255u], w[j]);
+    bar();
+    if (warp == 0) {
+      // lane owns digits 255 - 8 lane - i, i = 0..7 (descending): the first digit where the mass from the top reaches P
+      unsigned long long c[8], s = 0ull;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) { c[i] = hist[255 - 8 * lane - i]; s += c[i]; }
+      unsigned long long incl = s;
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long v = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += v;
+      }
+      if (shift == 24) P = (double)p * (double)__shfl_sync(0xffffffffu, incl, 31);
+      unsigned long long before = above + (incl - s);
+      const bool mine = (double)before < P && (double)(above + incl) >= P;
+      unsigned digit = 0u;
+      if (mine) {
+        bool found = false;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          if (!found && (double)(before + c[i]) >= P) { digit = 255u - 8u * lane - i; found = true; }
+          if (!found) before += c[i];
+        }
+        sel[0] = digit;
+      }
+      // the owning lane is unique: P <= W, and the mass from the top only grows
+      const unsigned owner = __ballot_sync(0xffffffffu, mine);
+      above = __shfl_sync(0xffffffffu, before, owner ? __ffs(owner) - 1 : 0);
+    }
+    bar();
+    prefix |= sel[0] << shift;
+    pmask |= 255u << shift;
+  }
+  return prefix;
+}
+
+// number of set flags over the 256 threads (integer, so independent of the combine order)
+template <class Bar>
+__device__ __forceinline__ int cta_count8(int v, int* si, Bar bar) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  v = __reduce_add_sync(0xffffffffu, v);
+  if (lane == 0) si[warp] = v;
+  bar();
+  v = si[0];
+#pragma unroll
+  for (int w = 1; w < 8; ++w) v += si[w];
+  bar();
+  return v;
+}
+
 // Block-wide (value, index) maximum with first-index ties, same combine order as the default draw; every thread gets the
 // index (0x7fffffff when no thread had a candidate).
 template <class Bar>
@@ -1096,33 +1166,41 @@ __device__ __forceinline__ long long cta_first_argmax(const float (&l)[8], float
 //   temperature 0: first-index argmax of l (q is not read);
 //   else s = l / temperature (IEEE division), codes below the k-th largest logit -> -inf, then the default draw
 //   argmax((exp(s - max s) / sum) / q) with first-index ties, over the kept codes only.
+//   top_p < 1 / min_p > 0 (ts_pixelcnn_sample_ctl) drop further codes before the sum: with e = exp(s - max s) of the
+//   codes top-k kept and the integer mass w = rint(e 2^32), top-p keeps the codes at or above nucleus_key, min-p those
+//   with e >= min_p.  kept_dst (may be null) receives the size of the final keep set (1 for a greedy draw).
 // At temperature 1 without truncation this is the default sampler's arithmetic step for step (s == l).
 // A temperature so small that max(l) / temperature overflows makes every p / q NaN, so no code wins the draw: the code is
 // then the greedy one, the limit of the tempered draw as the temperature goes to 0.  The returned code always lies in
 // [0, 2048): logits that are all NaN give code 0.
-// logp_dst (may be null) receives (l[code] - max l) - log(sum exp(l - max l)).  scratch: 16 + 256 + 2 words from red.
+// logp_dst (may be null) receives (l[code] - max l) - log(sum exp(l - max l)).  scratch: the first 578 words of red (64 of
+// reductions, then one histogram region that the count and the mass select use in turn, then 2 words of selection).
 template <class Bar>
-__device__ __forceinline__ long long draw_controlled(const float (&l)[8], const float (&q)[8], float temperature, int top_k, float* red,
-                                     float* logp_dst, Bar bar) {
+__device__ __forceinline__ long long draw_controlled(const float (&l)[8], const float (&q)[8], float temperature, int top_k, float top_p,
+                                     float min_p, float* red, float* logp_dst, int* kept_dst, Bar bar) {
   const int tid = threadIdx.x;
   float* sf = red;
   int* si = reinterpret_cast<int*>(red + 16);
   long long* scode = reinterpret_cast<long long*>(red + 32);
   unsigned* hist = reinterpret_cast<unsigned*>(red + 64);
-  unsigned* sel = reinterpret_cast<unsigned*>(red + 320);
+  unsigned long long* hist64 = reinterpret_cast<unsigned long long*>(red + 64);
+  unsigned* sel = reinterpret_cast<unsigned*>(red + 576);
   float mx = l[0];
 #pragma unroll
   for (int j = 1; j < 8; ++j) mx = fmaxf(mx, l[j]);
   mx = cta_max8(mx, sf, bar);
   const bool greedy = temperature == 0.f;
-  const bool truncate = !greedy && top_k > 0 && top_k < PIX_NCODE;
+  const bool nucleus = !greedy && top_p < 1.f, floor_p = !greedy && min_p > 0.f;
+  const bool truncate = !greedy && ((top_k > 0 && top_k < PIX_NCODE) || nucleus || floor_p);
   bool keep[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) keep[j] = true;
-  if (truncate) {
-    uint32_t key[8];
+  uint32_t key[8];
+  if (!greedy && ((top_k > 0 && top_k < PIX_NCODE) || nucleus)) {
 #pragma unroll
     for (int j = 0; j < 8; ++j) key[j] = logit_key(l[j]);
+  }
+  if (!greedy && top_k > 0 && top_k < PIX_NCODE) {
     const uint32_t kth = kth_largest_key(key, top_k, hist, sel, bar);
 #pragma unroll
     for (int j = 0; j < 8; ++j) keep[j] = key[j] >= kth;
@@ -1138,7 +1216,21 @@ __device__ __forceinline__ long long draw_controlled(const float (&l)[8], const 
     const float mxs = mx / temperature;
     float ex[8], sum = 0.f;
 #pragma unroll
-    for (int j = 0; j < 8; ++j) { ex[j] = keep[j] ? expf(l[j] / temperature - mxs) : 0.f; sum += ex[j]; }
+    for (int j = 0; j < 8; ++j) ex[j] = keep[j] ? expf(l[j] / temperature - mxs) : 0.f;
+    if (nucleus) {
+      unsigned long long w[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) w[j] = __float2ull_rn(ex[j] * 0x1p32f);   // exact scaling, round to nearest even
+      const uint32_t theta = nucleus_key(key, w, top_p, hist64, sel, bar);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) keep[j] = keep[j] && key[j] >= theta;
+    }
+    if (floor_p) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) keep[j] = keep[j] && ex[j] >= min_p;
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { ex[j] = keep[j] ? ex[j] : 0.f; sum += ex[j]; }
     sum = cta_sum8(sum, sf, bar);
     if (temperature == 1.f && !truncate) sum_raw = sum;   // s == l: the softmax denominator is the untempered one
 #pragma unroll
@@ -1153,6 +1245,13 @@ __device__ __forceinline__ long long draw_controlled(const float (&l)[8], const 
     if (code == 0x7fffffff) code = cta_first_argmax(l, sf, si, scode, bar);
   }
   if (code >= PIX_NCODE) code = 0;   // all logits NaN: keep the embedding gather inside the table
+  if (kept_dst) {
+    int n = 0;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) n += keep[j] ? 1 : 0;
+    n = cta_count8(n, si, bar);
+    if (tid == 0) *kept_dst = greedy ? 1 : n;
+  }
   if (logp_dst) {
     if (greedy || temperature != 1.f || truncate) {
       float s = 0.f;
@@ -1206,8 +1305,9 @@ __device__ void run_sample_task(const PixTask& t, const PixArgs& A, int r, int m
 #pragma unroll
         for (int j = 0; j < 8; ++j) qv[j] = QPRE ? qpre[j] : q[tid + 256 * j];
       }
-      float* lp = A.logp_out ? A.logp_out + ((size_t)m * (A.Ttot - A.T0) + (r - A.T0)) * 2 + c : nullptr;
-      code = draw_controlled(l, qv, A.temperature, A.top_k, red, lp, CtaBar());
+      const size_t at = ((size_t)m * (A.Ttot - A.T0) + (r - A.T0)) * 2 + c;
+      code = draw_controlled(l, qv, A.temperature, A.top_k, A.top_p, A.min_p, red, A.logp_out ? A.logp_out + at : nullptr,
+                             A.kept_out ? A.kept_out + at : nullptr, CtaBar());
     } else {
       code = A.pre[((size_t)m * A.T0 + r) * 2 + c];
     }
@@ -1476,6 +1576,7 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
   A.trace = P->d_trace; A.trace_row = P->trace_row;
   const SampleCtl c = ctl ? *ctl : SampleCtl();
   A.temperature = c.temperature; A.top_k = c.top_k; A.logp_out = c.logp_out;
+  A.top_p = c.top_p; A.min_p = c.min_p; A.kept_out = c.kept_out;
   if (e->pixel_mode == 0) {
     // A/B switch: 0 = burst loads + scalar FFMA, 4 = pipelined loads + scalar FFMA, 5 (default) = pipelined loads + paired FMAs (fma2)
     static const int pipe = getenv("TS_PIX_PIPE") ? atoi(getenv("TS_PIX_PIPE")) : 5;
@@ -1559,6 +1660,16 @@ void check_sample_ctl(const SampleCtl& c, const float* noise) {
     fail(TS_ERR_INVALID, "pixelcnn sample: temperature %g (must be finite and >= 0)", (double)c.temperature);
   if (c.top_k < 0 || c.top_k > PIX_NCODE) fail(TS_ERR_INVALID, "pixelcnn sample: top_k %d outside [0, %d]", c.top_k, PIX_NCODE);
   if (c.temperature > 0.f && !noise) fail(TS_ERR_INVALID, "pixelcnn sample: noise is NULL with temperature %g > 0", (double)c.temperature);
+  if (!(c.top_p > 0.f && c.top_p <= 1.f)) fail(TS_ERR_INVALID, "pixelcnn sample: top_p %g outside (0, 1]", (double)c.top_p);
+  if (!(c.min_p >= 0.f && c.min_p <= 1.f)) fail(TS_ERR_INVALID, "pixelcnn sample: min_p %g outside [0, 1]", (double)c.min_p);
+}
+
+SampleCtl sample_ctl_of(const ts_sample_ctl* c) {
+  if (!c) fail(TS_ERR_INVALID, "pixelcnn sample: ctl is NULL");
+  SampleCtl s;
+  s.temperature = c->temperature; s.top_k = c->top_k; s.top_p = c->top_p; s.min_p = c->min_p;
+  s.logp_out = c->logp_out; s.kept_out = c->kept_out;
+  return s;
 }
 
 }  // namespace ts
@@ -1718,10 +1829,16 @@ extern "C" int ts_pixelcnn_generate(ts_engine* e, const float* aud, const int64_
 extern "C" int ts_pixelcnn_sample(ts_engine* e, const float* aud, const int64_t* label, const float* noise,
                                   int64_t* idx_out, float* logits_out, int B, int T, const int64_t* pre_latents, int T0,
                                   float temperature, int top_k, float* logp_out, void* stream) {
+  const ts_sample_ctl ctl = {temperature, top_k, 1.f, 0.f, logp_out, nullptr};
+  return ts_pixelcnn_sample_ctl(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, &ctl, stream);
+}
+
+extern "C" int ts_pixelcnn_sample_ctl(ts_engine* e, const float* aud, const int64_t* label, const float* noise,
+                                      int64_t* idx_out, float* logits_out, int B, int T, const int64_t* pre_latents, int T0,
+                                      const ts_sample_ctl* ctl, void* stream) {
   TS_API_BEGIN(e)
-  SampleCtl ctl;
-  ctl.temperature = temperature; ctl.top_k = top_k; ctl.logp_out = logp_out;
-  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, &ctl);
+  const SampleCtl c = sample_ctl_of(ctl);
+  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, &c);
   TS_API_END(e)
 }
 

@@ -71,15 +71,21 @@ struct PixelPlan {
   int64_t timed_rows = 0, timed_launches = 0;
 };
 
-// Sampling controls of ts_pixelcnn_sample / ts_body_sample (include/talkshow_b200.h).  A call without them runs the
+// Sampling controls of ts_pixelcnn_sample_ctl / ts_body_sample_ctl (include/talkshow_b200.h).  A call without them runs the
 // default sampler kernels; a call with them runs the WARP instantiations, whose only difference is the draw.
 struct SampleCtl {
   float temperature = 1.f;   // > 0: softmax(l / temperature); 0: greedy (first-index argmax of l, noise unread)
   int top_k = 0;             // 0 or 2048: off; else keep codes with l >= the k-th largest logit
   float* logp_out = nullptr; // [B,T,2] log_softmax(l)[code] of the untempered, untruncated model, or null
+  float top_p = 1.f;         // < 1: nucleus sampling on integer masses (nucleus_key, pixelcnn.cu); 1: off
+  float min_p = 0.f;         // > 0: keep codes with exp(l / t - max l / t) >= min_p; 0: off
+  int* kept_out = nullptr;   // [B,T,2] size of each draw's final keep set, or null
 };
-// Validates the controls (TS_ERR_INVALID): temperature finite and >= 0, top_k in [0, 2048], noise given when sampling.
+// Validates the controls (TS_ERR_INVALID): temperature finite and >= 0, top_k in [0, 2048], top_p in (0, 1], min_p in
+// [0, 1], noise given when sampling.
 void check_sample_ctl(const SampleCtl& c, const float* noise);
+// The public struct as the internal one (TS_ERR_INVALID when null).
+SampleCtl sample_ctl_of(const ts_sample_ctl* c);
 
 // aud: AudioEncoder output, channel-last [B, T0+T, 256].  ctl = nullptr: the default sampler.
 void pixelcnn_generate_act(ts_engine* e, const Act3& aud, const int64_t* label, const float* noise, int64_t* idx_out,

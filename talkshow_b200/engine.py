@@ -17,9 +17,9 @@ PIX_TILE = 64  # samples per PixelCNN launch (csrc/pixelcnn.h PIX_MB)
 NCODE = 2048   # codes of the body prior
 
 
-def check_sample_controls(temperature, top_k):
+def check_sample_controls(temperature, top_k, top_p=1.0, min_p=0.0):
     """Validate the values of the sampler's controls (ValueError): temperature finite and >= 0 (0 = greedy decoding),
-    top_k an integer in [0, 2048] (0 = off)."""
+    top_k an integer in [0, 2048] (0 = off), top_p in (0, 1] (1 = off), min_p in [0, 1] (0 = off)."""
     try:
         t = float(temperature)
     except (TypeError, ValueError):
@@ -28,24 +28,49 @@ def check_sample_controls(temperature, top_k):
         raise ValueError("temperature must be finite and >= 0 (0 = greedy), got %r" % (temperature,))
     if isinstance(top_k, bool) or int(top_k) != top_k or not 0 <= int(top_k) <= NCODE:
         raise ValueError("top_k must be an integer in [0, %d] (0 = off), got %r" % (NCODE, top_k))
+    for name, v, ok in (("top_p", top_p, lambda x: 0 < x <= 1), ("min_p", min_p, lambda x: 0 <= x <= 1)):
+        try:
+            x = float(v)
+        except (TypeError, ValueError):
+            raise ValueError("%s must be a number, got %r" % (name, v))
+        # the engine takes the fp32 value: one that rounds out of the range (a top_p below the smallest float) is invalid too
+        if isinstance(v, bool) or not ok(x) or not ok(float(torch.tensor(x, dtype=torch.float32))):
+            raise ValueError("%s must lie in %s, got %r" % (name, "(0, 1] (1 = off)" if name == "top_p" else "[0, 1] (0 = off)", v))
 
 
-def sample_controls(temperature=1.0, top_k=0, keep_logp=False):
+def sample_controls(temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0):
     """Validated keyword arguments of ``Engine.pixelcnn_generate`` / ``body_generate`` for these controls; empty at the
-    defaults, so that those calls keep the default entry points (ts_pixelcnn_generate / ts_body_generate)."""
-    check_sample_controls(temperature, top_k)
-    if float(temperature) == 1.0 and not top_k and not keep_logp:
+    defaults, so that those calls keep the default entry points (ts_pixelcnn_generate / ts_body_generate).  ``top_p``,
+    ``min_p`` and ``want_kept`` appear only when nucleus or min-p truncation is on; the keep-set sizes are then asked for
+    together with the log-likelihoods."""
+    check_sample_controls(temperature, top_k, top_p, min_p)
+    nucleus = float(top_p) < 1.0 or float(min_p) > 0.0
+    if float(temperature) == 1.0 and not top_k and not keep_logp and not nucleus:
         return {}
-    return dict(temperature=temperature, top_k=top_k, want_logp=bool(keep_logp))
+    ctl = dict(temperature=temperature, top_k=top_k, want_logp=bool(keep_logp))
+    if nucleus:
+        ctl.update(top_p=top_p, min_p=min_p, want_kept=bool(keep_logp))
+    return ctl
 
 
-def _controlled(temperature, top_k, noise, want_logp):
-    """Engine side: validate the controls and the noise; True when the call goes to ts_pixelcnn_sample / ts_body_sample."""
-    check_sample_controls(temperature, top_k)
+def _controlled(temperature, top_k, noise, want_logp, top_p=1.0, min_p=0.0, want_kept=False):
+    """Engine side: validate the controls and the noise; True when the call leaves the default entry points."""
+    check_sample_controls(temperature, top_k, top_p, min_p)
     if noise is None and float(temperature) > 0:
         raise ValueError("sampling at temperature %g needs the noise tensor (only greedy decoding, temperature 0, "
                          "runs without)" % float(temperature))
-    return bool(sample_controls(temperature, top_k, want_logp))
+    return bool(sample_controls(temperature, top_k, want_logp, top_p, min_p)) or bool(want_kept)
+
+
+def _needs_ctl(top_p, min_p, want_kept):
+    """True when a controlled call needs ts_pixelcnn_sample_ctl / ts_body_sample_ctl: top_p, min_p or the keep-set sizes.
+    Every other controlled call stays on ts_pixelcnn_sample / ts_body_sample."""
+    return float(top_p) < 1.0 or float(min_p) > 0.0 or bool(want_kept)
+
+
+def _ctl_struct(temperature, top_k, top_p, min_p, logp, kept):
+    return _lib.ts_sample_ctl(float(temperature), int(top_k), float(top_p), float(min_p),
+                              None if logp is None else logp.data_ptr(), None if kept is None else kept.data_ptr())
 
 
 class Engine:
@@ -193,15 +218,19 @@ class Engine:
         return out
 
     def pixelcnn_generate(self, aud, label, noise, T=None, pre_latents=None, want_logits=False, temperature=1.0, top_k=0,
-                          want_logp=False):
+                          want_logp=False, top_p=1.0, min_p=0.0, want_kept=False):
         """GatedPixelCNN.generate: aud [B,256,T0+T], label [B], noise [2T,B,2048] -> codes [B,T,2]
         (+ logits [2T,B,2048]).  Batches above the 64-sample tile are chunked here.
 
         Sampling controls (ts_pixelcnn_sample): ``temperature`` (0 = greedy, noise may then be None), ``top_k``
         (0 = off), ``want_logp`` adds logp [B,T,2] = log_softmax(logits)[code] of the untempered model.  The result is
         codes, followed by logits when ``want_logits`` and logp when ``want_logp``.  The defaults call
-        ts_pixelcnn_generate."""
-        ctl = _controlled(temperature, top_k, noise, want_logp)
+        ts_pixelcnn_generate.
+
+        ``top_p`` (1 = off) and ``min_p`` (0 = off) truncate the draw further (nucleus / min-p sampling, in the order
+        temperature, top_k, top_p, min_p; ts_pixelcnn_sample_ctl); ``want_kept`` appends kept [B,T,2] int32, the number
+        of codes each draw chose among."""
+        ctl = _controlled(temperature, top_k, noise, want_logp, top_p, min_p, want_kept)
         aud = self._dev(aud, torch.float32)
         label = self._dev(label, torch.int64)
         noise = None if noise is None else self._dev(noise, torch.float32)
@@ -214,6 +243,7 @@ class Engine:
         codes = torch.empty(B, T, 2, dtype=torch.int64, device=self.device)
         logits = torch.empty(2 * T, B, 2048, device=self.device) if want_logits else None
         logp = torch.empty(B, T, 2, device=self.device) if want_logp else None
+        kept = torch.empty(B, T, 2, dtype=torch.int32, device=self.device) if want_kept else None
         aud_c = aud.shape[1]
         assert aud_c == 256, "AudioEncoder output has 256 channels"
         for b0 in range(0, B, PIX_TILE):
@@ -224,9 +254,13 @@ class Engine:
             cz = codes if full else torch.empty(nb, T, 2, dtype=torch.int64, device=self.device)
             lz = logits if (full or logits is None) else torch.empty(2 * T, nb, 2048, device=self.device)
             pz = logp if (full or logp is None) else torch.empty(nb, T, 2, device=self.device)
+            kz = kept if (full or kept is None) else torch.empty(nb, T, 2, dtype=torch.int32, device=self.device)
             args = (self.h, _lib.ptr(aud[b0:b1].contiguous()), _lib.ptr(label[b0:b1].contiguous()), _lib.ptr(nz),
                     _lib.ptr(cz), _lib.ptr(lz), nb, T, _lib.ptr(None if pre is None else pre[b0:b1].contiguous()), T0)
-            if ctl:
+            if ctl and _needs_ctl(top_p, min_p, want_kept):
+                c = _ctl_struct(temperature, top_k, top_p, min_p, pz, kz)
+                self._check(self.L.ts_pixelcnn_sample_ctl(*args, C.byref(c), self._s()), "ts_pixelcnn_sample_ctl")
+            elif ctl:
                 self._check(self.L.ts_pixelcnn_sample(*args, float(temperature), int(top_k), _lib.ptr(pz), self._s()),
                             "ts_pixelcnn_sample")
             else:
@@ -237,7 +271,9 @@ class Engine:
                     logits[:, b0:b1] = lz
                 if logp is not None:
                     logp[b0:b1] = pz
-        out = (codes,) + ((logits,) if want_logits else ()) + ((logp,) if want_logp else ())
+                if kept is not None:
+                    kept[b0:b1] = kz
+        out = (codes,) + ((logits,) if want_logits else ()) + ((logp,) if want_logp else ()) + ((kept,) if want_kept else ())
         return out if len(out) > 1 else codes
 
     def pixelcnn_logits(self, aud, label, codes):
@@ -361,10 +397,12 @@ class Engine:
                                            self._s()), "ts_face_forward")
         return out
 
-    def body_generate(self, mfcc, label, noise, want_codes=True, temperature=1.0, top_k=0, want_logp=False):
+    def body_generate(self, mfcc, label, noise, want_codes=True, temperature=1.0, top_k=0, want_logp=False, top_p=1.0,
+                      min_p=0.0, want_kept=False):
         """fused s2g_body_pixel core: mfcc [B,64,M] -> (codes [B,T,2], poses [B,4T,C]), C = 129 (258 for 6-D).
-        Sampling controls as in ``pixelcnn_generate`` (ts_body_sample); ``want_logp`` appends logp [B,T,2]."""
-        ctl = _controlled(temperature, top_k, noise, want_logp)
+        Sampling controls as in ``pixelcnn_generate`` (ts_body_sample, ts_body_sample_ctl); ``want_logp`` appends logp
+        [B,T,2], ``want_kept`` then kept [B,T,2] int32."""
+        ctl = _controlled(temperature, top_k, noise, want_logp, top_p, min_p, want_kept)
         mfcc = self._dev(mfcc, torch.float32)
         label = self._dev(label, torch.int64)
         noise = None if noise is None else self._dev(noise, torch.float32)
@@ -375,19 +413,24 @@ class Engine:
         codes = torch.empty(B, T, 2, dtype=torch.int64, device=self.device) if want_codes else None
         poses = torch.empty(B, 4 * T, self.vq_dim(0) + self.vq_dim(1), device=self.device)
         logp = torch.empty(B, T, 2, device=self.device) if want_logp else None
+        kept = torch.empty(B, T, 2, dtype=torch.int32, device=self.device) if want_kept else None
         for b0 in range(0, B, PIX_TILE):
             b1 = min(B, b0 + PIX_TILE)
             full = (b1 - b0) == B
             nz = noise if (full or noise is None) else noise[:, b0:b1].contiguous()
             args = (self.h, _lib.ptr(mfcc[b0:b1]), _lib.ptr(label[b0:b1]), _lib.ptr(nz),
                     _lib.ptr(None if codes is None else codes[b0:b1]), _lib.ptr(poses[b0:b1]), b1 - b0, M)
-            if ctl:
+            if ctl and _needs_ctl(top_p, min_p, want_kept):
+                c = _ctl_struct(temperature, top_k, top_p, min_p, None if logp is None else logp[b0:b1],
+                                None if kept is None else kept[b0:b1])
+                self._check(self.L.ts_body_sample_ctl(*args, C.byref(c), self._s()), "ts_body_sample_ctl")
+            elif ctl:
                 self._check(self.L.ts_body_sample(*args, float(temperature), int(top_k),
                                                   _lib.ptr(None if logp is None else logp[b0:b1]), self._s()),
                             "ts_body_sample")
             else:
                 self._check(self.L.ts_body_generate(*args, self._s()), "ts_body_generate")
-        return (codes, poses, logp) if want_logp else (codes, poses)
+        return (codes, poses) + ((logp,) if want_logp else ()) + ((kept,) if want_kept else ())
 
     # -- the single collective of the path, inside the library (ts_allgather over a dlopen'ed NCCL) ----------------
     @staticmethod

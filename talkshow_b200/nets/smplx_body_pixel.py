@@ -110,7 +110,7 @@ class TrainWrapper:
                        continuity=False, id=None, fps=15, sr=22000, B=1, am=None, am_sr=None, frame=0, **kwargs):
         """(aud_fn) -> generated motion, numpy (B, F, 129).  Reference: :232-289."""
         assert self.args.infer, "train mode"
-        ctl = {k: kwargs[k] for k in ("temperature", "top_k", "keep_logp") if k in kwargs}
+        ctl = {k: kwargs[k] for k in ("temperature", "top_k", "keep_logp", "top_p", "min_p") if k in kwargs}
         if continuity:
             return self._infer_continuity(aud_fn, id, fps, sr, B, **ctl)
         if torch.is_tensor(aud_fn) or isinstance(aud_fn, np.ndarray):
@@ -125,43 +125,47 @@ class TrainWrapper:
         label = torch.tensor([0]) if id is None else id.reshape(-1).repeat(B)[:B] if id.numel() == 1 else id
         return self.generate(mfcc, label, noise_fn=kwargs.get("noise_fn"), **ctl).cpu().numpy()
 
-    def generate(self, aud, id, frame_num=0, noise_fn=None, temperature=1.0, top_k=0, keep_logp=False):
+    def generate(self, aud, id, frame_num=0, noise_fn=None, temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0):
         """tensor API (:306-326): aud [B,64,M] features, id [B] -> torch (B, F, 129) on the device.
         (The reference's version passes decode()'s tuple to torch.cat and raises; this returns the
         tensor its infer_on_audio builds.)
 
         Sampling controls of the prior (Engine.pixelcnn_generate): ``temperature`` (0 = greedy decoding, which draws no
         noise), ``top_k`` (0 = off); ``keep_logp`` keeps each draw's log-likelihood under the untempered prior as
-        self.last_logp [B,T,2].  The defaults draw exactly like the reference."""
+        self.last_logp [B,T,2].  ``top_p`` (1 = off) and ``min_p`` (0 = off) add nucleus and min-p truncation; with
+        ``keep_logp`` the number of codes each such draw chose among is kept as self.last_kept [B,T,2] (None when both are
+        off).  The defaults draw exactly like the reference."""
         mfcc = aud.to(torch.float32)
         B, _, M = mfcc.shape
         T = self.engine.latent_rows(M)
-        noise = self._draw_noise(T, B, noise_fn, temperature, top_k)
-        out = self.engine.body_generate(mfcc, id.to(torch.int64), noise, **sample_controls(temperature, top_k, keep_logp))
+        noise = self._draw_noise(T, B, noise_fn, temperature, top_k, top_p, min_p)
+        ctl = sample_controls(temperature, top_k, keep_logp, top_p, min_p)
+        out = self.engine.body_generate(mfcc, id.to(torch.int64), noise, **ctl)
         self.last_codes, poses = out[0], out[1]
         self.last_logp = out[2] if keep_logp else None
+        self.last_kept = out[3] if ctl.get("want_kept") else None
         return poses
 
-    def _draw_noise(self, T, B, noise_fn, temperature, top_k):
+    def _draw_noise(self, T, B, noise_fn, temperature, top_k, top_p=1.0, min_p=0.0):
         """[2T,B,2048] Exp(1) draws (RNG contract), or None for greedy decoding (controls validated first)."""
-        check_sample_controls(temperature, top_k)
+        check_sample_controls(temperature, top_k, top_p, min_p)
         if float(temperature) == 0:
             return None
         return self._noise(T, B) if noise_fn is None else noise_fn(T, B)
 
     def infer(self, aud_feat, frame, id, B, pre_latents=None, pre_audio=None, pre_pose=None, noise_fn=None,
-              temperature=1.0, top_k=0, keep_logp=False):
+              temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0):
         """The reference's inner call (:291-304): aud_feat [B,M,64] (time-major features of ONE chunk) ->
         (latents [B,T,2], audio [B,256,T,2], body [B,39,4T], hand [B,90,4T]).  ``pre_latents`` / ``pre_audio`` (the first
         two results of the previous chunk's call) condition the sampler on that chunk (GatedPixelCNN.generate :158-165);
         ``pre_pose`` is accepted and unused like in the reference, whose Decoder.forward ignores ``pre_state``
         (nets/spg/vqvae_1d.py:139-149) — each chunk is decoded on its own.  Sampling controls as in ``generate``; with
-        ``keep_logp`` the chunk's logp [B,T,2] is kept as self.last_logp."""
+        ``keep_logp`` the chunk's logp [B,T,2] is kept as self.last_logp (and its keep-set sizes as self.last_kept)."""
         a = self.engine.audio_encode(aud_feat.transpose(1, 2).contiguous())            # [B,256,T]
         T = a.shape[2]
         label = id.reshape(-1)
-        noise = self._draw_noise(T, B, noise_fn, temperature, top_k)
-        ctl = sample_controls(temperature, top_k, keep_logp)
+        noise = self._draw_noise(T, B, noise_fn, temperature, top_k, top_p, min_p)
+        ctl = sample_controls(temperature, top_k, keep_logp, top_p, min_p)
         if pre_latents is None:
             out = self.engine.pixelcnn_generate(a, label, noise, **ctl)
         else:
@@ -170,6 +174,7 @@ class TrainWrapper:
                                                 pre_latents=pre_latents, **ctl)
         latents = out[0] if keep_logp else out
         self.last_logp = out[1] if keep_logp else None
+        self.last_kept = out[2] if ctl.get("want_kept") else None
         body = self.engine.vq_decode(0, latents[..., 0].contiguous())
         hand = self.engine.vq_decode(1, latents[..., 1].contiguous())
         return latents, a.unsqueeze(-1).repeat(1, 1, 1, 2), body, hand
@@ -183,10 +188,11 @@ class TrainWrapper:
         label = torch.tensor([0]) if id is None else id.reshape(-1).repeat(B)
         pre_pose = {"b": None, "h": None}
         lat0, audio0, body_0, hand_0 = self.infer(feat[:, :gap], 0, label, B, pre_pose=pre_pose, keep_logp=keep_logp, **ctl)
-        logp0 = self.last_logp
+        logp0, kept0 = self.last_logp, self.last_kept
         pre_pose["b"], pre_pose["h"] = body_0[:, :, -4:].transpose(1, 2), hand_0[:, :, -4:].transpose(1, 2)
         lat1, _, body_1, hand_1 = self.infer(feat[:, gap:], 0, label, B, lat0, audio0, pre_pose, keep_logp=keep_logp, **ctl)
         self.last_codes = torch.cat([lat0, lat1], 1)
         self.last_logp = torch.cat([logp0, self.last_logp], 1) if keep_logp else None
+        self.last_kept = torch.cat([kept0, self.last_kept], 1) if kept0 is not None else None
         body, hand = torch.cat([body_0, body_1], 2), torch.cat([hand_0, hand_1], 2)
         return torch.cat([body, hand], 1).transpose(1, 2).cpu().numpy()

@@ -78,16 +78,17 @@ class WholeBody:
             self.e2 = None
 
     def generate(self, mfcc, wave, label, noise=None, stand=False, per_step_noise=True, temperature=1.0, top_k=0,
-                 keep_logp=False):
+                 keep_logp=False, top_p=1.0, min_p=0.0):
         """mfcc [B,64,M], wave [B,N] (16 kHz), label [B] on the device -> poses [B,F,265] (device).
         F = N*30//16000 face frames; the body (4*T frames) is padded/truncated to F like demo.py:207-211.
         Sampling controls of the body prior as in s2g_body_pixel.generate: ``temperature`` (0 = greedy, no noise is
-        drawn), ``top_k``; ``keep_logp`` keeps each draw's log-likelihood under the untempered prior as
-        self.last_logp [B,T,2]."""
+        drawn), ``top_k``, ``top_p``, ``min_p``; ``keep_logp`` keeps each draw's log-likelihood under the untempered prior
+        as self.last_logp [B,T,2] and, with top_p or min_p on, the size of its keep set as self.last_kept [B,T,2]."""
         B, _, M = mfcc.shape
         frame = wave.shape[1] * 30 // 16000
         T = self.e.latent_rows(M)
-        ctl = sample_controls(temperature, top_k, keep_logp)
+        ctl = sample_controls(temperature, top_k, keep_logp, top_p, min_p)
+        want_kept = bool(ctl.get("want_kept"))
         if noise is None and float(temperature) > 0:
             noise = draw_sampler_noise(T, B, self.device, per_step=per_step_noise)
         idz = torch.zeros(B, 4, device=self.device)                    # demo.py:173-181: id not passed
@@ -100,11 +101,14 @@ class WholeBody:
                 out = self.e2.body_generate(mfcc, label, noise, want_codes=False, **ctl)
             body = out[1]
             self.last_logp = out[2] if keep_logp else None
+            self.last_kept = out[3] if want_kept else None
             face = self.e.face_forward(wave, idz, frame)
             cur.wait_stream(self._side)
             body.record_stream(cur)                                      # allocated on the side stream, consumed here
             if keep_logp:
                 self.last_logp.record_stream(cur)
+            if want_kept:
+                self.last_kept.record_stream(cur)
             for t in (mfcc, label, noise):
                 if torch.is_tensor(t) and t.is_cuda:
                     t.record_stream(self._side)                          # allocated here, consumed on the side stream
@@ -113,6 +117,7 @@ class WholeBody:
         face = self.e.face_forward(wave, idz, frame)
         out = self.e.body_generate(mfcc, label, noise, want_codes=False, **ctl)
         self.last_logp = out[2] if keep_logp else None
+        self.last_kept = out[3] if want_kept else None
         return self.e.assemble_pose(face, out[1], stand)
 
     def evaluate(self, bat):
@@ -149,19 +154,22 @@ class WholeBody:
         return None, dict(face_losses, **vq_losses, ce_loss=float(nll.double().mean()))
 
     def generate_sharded(self, mfcc, wave, label, rank, world, noise_full=None, seed=None, stand=False, gather=True,
-                         group=None, temperature=1.0, top_k=0, keep_logp=False):
+                         group=None, temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0):
         """Multi-GPU form of ``generate`` whose RESULT DOES NOT DEPEND ON ``world`` (SURVEY.md §8e): the arguments are
         the FULL batch (host or device tensors, identical on every rank), the sampler noise is drawn for the full batch in
         the reference's order — ``noise_full`` [2T,B,2048], or drawn here from ``seed`` on this rank's device generator
         (same seed on every rank gives every rank the same stream) — and rank r keeps the slice of its contiguous shard
         ``shard_range(B, r, world)``.  Each rank runs its shard; ONE all-gather rebuilds [B,F,265] everywhere.
         Sampling controls as in ``generate`` (greedy decoding draws no noise); with ``keep_logp`` self.last_logp holds
-        this rank's shard."""
+        this rank's shard (and self.last_kept, as in ``generate``)."""
         B, _, M = mfcc.shape
         lo, hi = shard_range(B, rank, world)
         T = self.e.latent_rows(M)
         # validated before any noise is drawn; generate() gets the controls only when they differ from the defaults
-        ctl = dict(temperature=temperature, top_k=top_k, keep_logp=keep_logp) if sample_controls(temperature, top_k, keep_logp) else {}
+        sc = sample_controls(temperature, top_k, keep_logp, top_p, min_p)
+        ctl = dict(temperature=temperature, top_k=top_k, keep_logp=keep_logp) if sc else {}
+        if "top_p" in sc:
+            ctl.update(top_p=top_p, min_p=min_p)
         if noise_full is None and float(temperature) > 0:
             g = None
             if seed is not None:
@@ -172,6 +180,7 @@ class WholeBody:
             frame = wave.shape[1] * 30 // 16000
             local = torch.empty(0, frame, 265, device=self.device)
             self.last_logp = torch.empty(0, T, 2, device=self.device) if keep_logp else None
+            self.last_kept = torch.empty(0, T, 2, dtype=torch.int32, device=self.device) if sc.get("want_kept") else None
         else:
             dev = lambda t: t[lo:hi].to(self.device, non_blocking=True)
             nz = None if noise_full is None else noise_full[:, lo:hi].to(self.device).contiguous()
