@@ -293,6 +293,38 @@ typedef struct ts_debug_conv {
 } ts_debug_conv;
 int ts_debug_conv1d(ts_engine* e, const ts_debug_conv* a, const float* x, const float* W_host, const float* bias_host,
                     const float* res, float* y, void* y_plane_hi, void* y_plane_lo, void* stream);
+/* The face regressor's self-attention through one kernel (unit tests), as the face forward runs it: 12 heads of 64,
+ *   out(b, t, 64 h + d) = sum_j softmax_j(q(b, t, h) . k(b, j, h) / 8) v(b, j, h)[d]
+ * with qkv [B,T,2304] device fp32 in the layout of the fused projection, rows [q(768) | k(768) | v(768)], head h at
+ * columns 64 h of each block.  qkv is staged in the workspace with 64 NaN rows after the last item (no kernel reads them).
+ *   kernel: -1 the one the face forward runs for T frames (TS_ATT_MMA, default: 3 up to 384 frames, 4 beyond), 0 FFMA
+ *     attention_kernel (T <= 3136), 1 tf32 3xTF32 attention_mma_kernel, 2 fp16-split attention_mma16_kernel,
+ *     3 attention_mma16p_kernel (K / V resident, split once per CTA; 1, 2 and 3 hold T <= 384), 4 attention_mma16t_kernel
+ *     (K / V staged `chunk` keys at a time, any T);
+ *   chunk: kernel 4 only, a multiple of 64 in [64, 384]; 0 = the face forward's 320;
+ *   out_format: 0 fp32 in out; 1 the 3xTF32 (hi, lo) pair of ts_set_tensor_cores(e, 1) in plane_hi / plane_lo (fp32,
+ *     out unused, may be NULL); 2 (kernels 3 and 4, the default mode 6) fp32 in out plus its fp16 planes
+ *     h = fp16(o), l = fp16(o - h) (uint16) in plane_hi / plane_lo.
+ * Output buffers are [B,T,768]; their contents are copied in before the kernel and back after it.
+ * Input contract of the fp16-split kernels (2, 3, 4): |q| / 8, |k| and |v| below 65504; every operand is carried to 22
+ * significant bits only while its low fp16 plane is normal -- values below about 2^-3 pay an absolute error of up to
+ * 2^-25, and below 2^-14 the high plane itself is subnormal.  Kernels 3 and 4 give the same bits at every T kernel 3 holds.
+ * Returns TS_ERR_INVALID, before any launch, for a kernel that cannot hold T, a chunk off the grid above, or format 2 on
+ * kernels 0 - 2.  The engine's ts_set_tensor_cores setting is unchanged afterwards. */
+typedef struct ts_debug_att {
+  int32_t kernel, B, T, chunk, out_format;
+} ts_debug_att;
+int ts_debug_attention(ts_engine* e, const ts_debug_att* a, const float* qkv, float* out, void* plane_hi, void* plane_lo,
+                       void* stream);
+/* The face regressor's positional conv (pos_conv_embed: Conv1d(768, 768, 128, padding 64, groups 16), last output
+ * dropped, then erf-GELU) through one kernel (unit tests): x [B,T,768] device fp32, staged with the face forward's 64 zero
+ * rows before and after every item; W_host [768,48,128] (torch layout) and bias_host [768] host fp32, packed as
+ * ts_load_face packs them; y [B,T,768] device fp32, copied in before the kernel and back after it.
+ *   mode 6 or 1: posconv_mma_kernel (fp16-split HMMA, weights pre-split and scaled per layer); 0: the FFMA GEMM with one
+ *   grid slice per group.
+ * The engine's ts_set_tensor_cores setting is unchanged afterwards. */
+int ts_debug_posconv(ts_engine* e, int mode, const float* x, const float* W_host, const float* bias_host, float* y, int B,
+                     int T, void* stream);
 /* Dense-contraction kernel for the face network and the VQ decoder (csrc/gemm_tc.cu):
  *   6 (default) Hopper wgmma kernel (128x128 tile) on two-term fp16-split operands (three products per MAC: fp32-grade
  *       results at twice the tf32 rate; operands must stay below 65504 in magnitude -- weights are pre-scaled per layer),

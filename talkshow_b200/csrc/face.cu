@@ -671,6 +671,93 @@ __global__ void __launch_bounds__(ATT_WARPS * 32, 1) attention_mma16_kernel(cons
 // fragment register is one 32-bit shared load (two adjacent d for K, two adjacent keys for V^T) and the inner
 // loops are 4 LDS + 3 HMMA per product triple.  Same bytes of shared memory as the fp32 copies.
 constexpr int ATT_KW = 36;    // K plane row stride in 32-bit words (72 halves): fragment loads conflict-free
+
+// One 64-key block of the online softmax, the step of both kernels below: scores of the warp's 16 query rows (fragments
+// qh / ql, already scaled) against keys [kb, kb + 64) of the shared planes -- clip keys key0 + kb + ... --, keys >= T
+// masked, the running max / sum update, O += P V.  The tensor core's fp32 accumulator truncates, so P V of the block
+// accumulates into a fresh fragment (12 MMAs deep) that is added to O with round-to-nearest adds: the truncation does not
+// build up with the clip length, and a block gives the same bits however the keys are staged (whole clip or chunks).
+__device__ __forceinline__ void att16_block(const uint32_t* Kh, const uint32_t* Kl, const uint32_t* Vh, const uint32_t* Vl, int VW, int kb,
+                                            int key0, int T, const uint32_t (&qh)[4][4], const uint32_t (&ql)[4][4], float (&o)[8][4],
+                                            float& m_a, float& m_b, float& l_a, float& l_b, int g, int t) {
+  float sc[8][4];
+#pragma unroll
+  for (int nt = 0; nt < 8; ++nt) sc[nt][0] = sc[nt][1] = sc[nt][2] = sc[nt][3] = 0.f;
+  // b0 = K[key = kb + 8 nt + g][d = 16 ks + 2t, +1] = word (8 ks + t) of the key's row, b1 = word (8 ks + t + 4)
+  // (the three products of one accumulator are issued a whole pass apart, so dependent HMMAs never queue back to back)
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) {
+    uint32_t bh0[8], bh1[8], bl0[8], bl1[8];
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+      const int w = (kb + nt * 8 + g) * ATT_KW + ks * 8 + t;
+      bh0[nt] = Kh[w]; bh1[nt] = Kh[w + 4]; bl0[nt] = Kl[w]; bl1[nt] = Kl[w + 4];
+    }
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) mma_f16(sc[nt], ql[ks], bh0[nt], bh1[nt]);
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) mma_f16(sc[nt], qh[ks], bl0[nt], bl1[nt]);
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) mma_f16(sc[nt], qh[ks], bh0[nt], bh1[nt]);
+  }
+  float mx_a = -INFINITY, mx_b = -INFINITY;
+#pragma unroll
+  for (int nt = 0; nt < 8; ++nt) {
+    const int key = key0 + kb + nt * 8 + 2 * t;
+    if (key >= T) sc[nt][0] = sc[nt][2] = -INFINITY;
+    if (key + 1 >= T) sc[nt][1] = sc[nt][3] = -INFINITY;
+    mx_a = fmaxf(mx_a, fmaxf(sc[nt][0], sc[nt][1]));
+    mx_b = fmaxf(mx_b, fmaxf(sc[nt][2], sc[nt][3]));
+  }
+  mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 1));
+  mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 2));
+  mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 1));
+  mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 2));
+  const float mn_a = fmaxf(m_a, mx_a), mn_b = fmaxf(m_b, mx_b);   // finite: every block holds a key < T
+  const float ca = expf(m_a - mn_a), cb = expf(m_b - mn_b);
+  m_a = mn_a; m_b = mn_b;
+  l_a *= ca; l_b *= cb;
+#pragma unroll
+  for (int dt = 0; dt < 8; ++dt) { o[dt][0] *= ca; o[dt][1] *= ca; o[dt][2] *= cb; o[dt][3] *= cb; }
+  float oc[8][4];
+#pragma unroll
+  for (int dt = 0; dt < 8; ++dt) oc[dt][0] = oc[dt][1] = oc[dt][2] = oc[dt][3] = 0.f;
+  // b0 = V^T[d = 8 dt + g][keys kb + 16 j2 + 2t, +1] = word ((kb + 16 j2) / 2 + t) of row d, b1 = that + 4
+#pragma unroll
+  for (int j2 = 0; j2 < 4; ++j2) {
+    if (key0 + kb + j2 * 16 >= T) break;     // whole 16-key step is padding (warp-uniform)
+    float p[8];
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      p[q * 4 + 0] = expf(sc[2 * j2 + q][0] - mn_a);
+      p[q * 4 + 1] = expf(sc[2 * j2 + q][1] - mn_a);
+      p[q * 4 + 2] = expf(sc[2 * j2 + q][2] - mn_b);
+      p[q * 4 + 3] = expf(sc[2 * j2 + q][3] - mn_b);
+    }
+    l_a += (p[0] + p[1]) + (p[4] + p[5]);
+    l_b += (p[2] + p[3]) + (p[6] + p[7]);
+    uint32_t ph[4], pl[4];
+    split_h2(p[0] * 1024.f, p[1] * 1024.f, ph[0], pl[0]);
+    split_h2(p[2] * 1024.f, p[3] * 1024.f, ph[1], pl[1]);
+    split_h2(p[4] * 1024.f, p[5] * 1024.f, ph[2], pl[2]);
+    split_h2(p[6] * 1024.f, p[7] * 1024.f, ph[3], pl[3]);
+    uint32_t bh0[8], bh1[8], bl0[8], bl1[8];
+#pragma unroll
+    for (int dt = 0; dt < 8; ++dt) {
+      const int w = (dt * 8 + g) * VW + (kb >> 1) + j2 * 8 + t;
+      bh0[dt] = Vh[w]; bh1[dt] = Vh[w + 4]; bl0[dt] = Vl[w]; bl1[dt] = Vl[w + 4];
+    }
+#pragma unroll
+    for (int dt = 0; dt < 8; ++dt) mma_f16(oc[dt], pl, bh0[dt], bh1[dt]);
+#pragma unroll
+    for (int dt = 0; dt < 8; ++dt) mma_f16(oc[dt], ph, bl0[dt], bl1[dt]);
+#pragma unroll
+    for (int dt = 0; dt < 8; ++dt) mma_f16(oc[dt], ph, bh0[dt], bh1[dt]);
+  }
+#pragma unroll
+  for (int dt = 0; dt < 8; ++dt) { o[dt][0] += oc[dt][0]; o[dt][1] += oc[dt][1]; o[dt][2] += oc[dt][2]; o[dt][3] += oc[dt][3]; }
+}
+
 __global__ void __launch_bounds__(ATT_WARPS * 32, 1) attention_mma16p_kernel(const float* __restrict__ qkv, float* __restrict__ out,
                                                                              float* __restrict__ out_lo, unsigned short* __restrict__ o_h16,
                                                                              unsigned short* __restrict__ o_l16, int T, int H, float scale) {
@@ -730,79 +817,7 @@ __global__ void __launch_bounds__(ATT_WARPS * 32, 1) attention_mma16p_kernel(con
 #pragma unroll
     for (int dt = 0; dt < 8; ++dt) o[dt][0] = o[dt][1] = o[dt][2] = o[dt][3] = 0.f;
     float m_a = -INFINITY, m_b = -INFINITY, l_a = 0.f, l_b = 0.f;
-    for (int kb = 0; kb < Tp; kb += 64) {
-      float sc[8][4];
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt) sc[nt][0] = sc[nt][1] = sc[nt][2] = sc[nt][3] = 0.f;
-      // b0 = K[key = kb + 8 nt + g][d = 16 ks + 2t, +1] = word (8 ks + t) of the key's row, b1 = word (8 ks + t + 4)
-      // (the three products of one accumulator are issued a whole pass apart, so dependent HMMAs never queue back to back)
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
-        uint32_t bh0[8], bh1[8], bl0[8], bl1[8];
-#pragma unroll
-        for (int nt = 0; nt < 8; ++nt) {
-          const int w = (kb + nt * 8 + g) * ATT_KW + ks * 8 + t;
-          bh0[nt] = Kh[w]; bh1[nt] = Kh[w + 4]; bl0[nt] = Kl[w]; bl1[nt] = Kl[w + 4];
-        }
-#pragma unroll
-        for (int nt = 0; nt < 8; ++nt) mma_f16(sc[nt], ql[ks], bh0[nt], bh1[nt]);
-#pragma unroll
-        for (int nt = 0; nt < 8; ++nt) mma_f16(sc[nt], qh[ks], bl0[nt], bl1[nt]);
-#pragma unroll
-        for (int nt = 0; nt < 8; ++nt) mma_f16(sc[nt], qh[ks], bh0[nt], bh1[nt]);
-      }
-      float mx_a = -INFINITY, mx_b = -INFINITY;
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt) {
-        const int key = kb + nt * 8 + 2 * t;
-        if (key >= T) sc[nt][0] = sc[nt][2] = -INFINITY;
-        if (key + 1 >= T) sc[nt][1] = sc[nt][3] = -INFINITY;
-        mx_a = fmaxf(mx_a, fmaxf(sc[nt][0], sc[nt][1]));
-        mx_b = fmaxf(mx_b, fmaxf(sc[nt][2], sc[nt][3]));
-      }
-      mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 1));
-      mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 2));
-      mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 1));
-      mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 2));
-      const float mn_a = fmaxf(m_a, mx_a), mn_b = fmaxf(m_b, mx_b);
-      const float ca = expf(m_a - mn_a), cb = expf(m_b - mn_b);
-      m_a = mn_a; m_b = mn_b;
-      l_a *= ca; l_b *= cb;
-#pragma unroll
-      for (int dt = 0; dt < 8; ++dt) { o[dt][0] *= ca; o[dt][1] *= ca; o[dt][2] *= cb; o[dt][3] *= cb; }
-      // b0 = V^T[d = 8 dt + g][keys kb + 16 j2 + 2t, +1] = word ((kb + 16 j2) / 2 + t) of row d, b1 = that + 4
-#pragma unroll
-      for (int j2 = 0; j2 < 4; ++j2) {
-        if (kb + j2 * 16 >= T) break;
-        float p[8];
-#pragma unroll
-        for (int q = 0; q < 2; ++q) {
-          p[q * 4 + 0] = expf(sc[2 * j2 + q][0] - mn_a);
-          p[q * 4 + 1] = expf(sc[2 * j2 + q][1] - mn_a);
-          p[q * 4 + 2] = expf(sc[2 * j2 + q][2] - mn_b);
-          p[q * 4 + 3] = expf(sc[2 * j2 + q][3] - mn_b);
-        }
-        l_a += (p[0] + p[1]) + (p[4] + p[5]);
-        l_b += (p[2] + p[3]) + (p[6] + p[7]);
-        uint32_t ph[4], pl[4];
-        split_h2(p[0] * 1024.f, p[1] * 1024.f, ph[0], pl[0]);
-        split_h2(p[2] * 1024.f, p[3] * 1024.f, ph[1], pl[1]);
-        split_h2(p[4] * 1024.f, p[5] * 1024.f, ph[2], pl[2]);
-        split_h2(p[6] * 1024.f, p[7] * 1024.f, ph[3], pl[3]);
-        uint32_t bh0[8], bh1[8], bl0[8], bl1[8];
-#pragma unroll
-        for (int dt = 0; dt < 8; ++dt) {
-          const int w = (dt * 8 + g) * VW + (kb >> 1) + j2 * 8 + t;
-          bh0[dt] = Vh[w]; bh1[dt] = Vh[w + 4]; bl0[dt] = Vl[w]; bl1[dt] = Vl[w + 4];
-        }
-#pragma unroll
-        for (int dt = 0; dt < 8; ++dt) mma_f16(o[dt], pl, bh0[dt], bh1[dt]);
-#pragma unroll
-        for (int dt = 0; dt < 8; ++dt) mma_f16(o[dt], ph, bl0[dt], bl1[dt]);
-#pragma unroll
-        for (int dt = 0; dt < 8; ++dt) mma_f16(o[dt], ph, bh0[dt], bh1[dt]);
-      }
-    }
+    for (int kb = 0; kb < Tp; kb += 64) att16_block(Kh, Kl, Vh, Vl, VW, kb, 0, T, qh, ql, o, m_a, m_b, l_a, l_b, g, t);
     l_a += __shfl_xor_sync(0xffffffffu, l_a, 1);
     l_a += __shfl_xor_sync(0xffffffffu, l_a, 2);
     l_b += __shfl_xor_sync(0xffffffffu, l_b, 1);
@@ -835,7 +850,7 @@ __global__ void __launch_bounds__(ATT_WARPS * 32, 1) attention_mma16p_kernel(con
   }
 }
 
-// Same arithmetic, KV-TILED for long clips (flash-attention style): the keys / values of a head are staged CH at a time,
+// Same arithmetic (att16_block: the same bits as the resident kernel at every T it can hold), KV-TILED for long clips (flash-attention style): the keys / values of a head are staged CH at a time,
 // every warp owns ONE 16-row query block and keeps its online-softmax state in registers across the chunks; grid =
 // (clip x head, query tiles of 16 x ATT_WARPS rows).  No limit on the clip length (the resident variant above needs the
 // whole sequence in shared memory: <= 384 frames = 12.8 s).
@@ -902,86 +917,7 @@ __global__ void __launch_bounds__(ATT_WARPS * 32, 1) attention_mma16t_kernel(con
       Vl[d * VW + kp] = lo;
     }
       __syncthreads();
-      for (int kb = 0; live && kb < Tp && c0 + kb < T; kb += 64) {
-        float sc[8][4];
-  #pragma unroll
-        for (int nt = 0; nt < 8; ++nt) sc[nt][0] = sc[nt][1] = sc[nt][2] = sc[nt][3] = 0.f;
-        // b0 = K[key = kb + 8 nt + g][d = 16 ks + 2t, +1] = word (8 ks + t) of the key's row, b1 = word (8 ks + t + 4)
-        // (the three products of one accumulator are issued a whole pass apart, so dependent HMMAs never queue back to back)
-  #pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {
-          uint32_t bh0[8], bh1[8], bl0[8], bl1[8];
-  #pragma unroll
-          for (int nt = 0; nt < 8; ++nt) {
-            const int w = (kb + nt * 8 + g) * ATT_KW + ks * 8 + t;
-            bh0[nt] = Kh[w]; bh1[nt] = Kh[w + 4]; bl0[nt] = Kl[w]; bl1[nt] = Kl[w + 4];
-          }
-  #pragma unroll
-          for (int nt = 0; nt < 8; ++nt) mma_f16(sc[nt], ql[ks], bh0[nt], bh1[nt]);
-  #pragma unroll
-          for (int nt = 0; nt < 8; ++nt) mma_f16(sc[nt], qh[ks], bl0[nt], bl1[nt]);
-  #pragma unroll
-          for (int nt = 0; nt < 8; ++nt) mma_f16(sc[nt], qh[ks], bh0[nt], bh1[nt]);
-        }
-        float mx_a = -INFINITY, mx_b = -INFINITY;
-  #pragma unroll
-        for (int nt = 0; nt < 8; ++nt) {
-          const int key = c0 + kb + nt * 8 + 2 * t;
-          if (key >= T) sc[nt][0] = sc[nt][2] = -INFINITY;
-          if (key + 1 >= T) sc[nt][1] = sc[nt][3] = -INFINITY;
-          mx_a = fmaxf(mx_a, fmaxf(sc[nt][0], sc[nt][1]));
-          mx_b = fmaxf(mx_b, fmaxf(sc[nt][2], sc[nt][3]));
-        }
-        mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 1));
-        mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 2));
-        mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 1));
-        mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 2));
-        const float mn_a = fmaxf(m_a, mx_a), mn_b = fmaxf(m_b, mx_b);
-        const float ca = expf(m_a - mn_a), cb = expf(m_b - mn_b);
-        m_a = mn_a; m_b = mn_b;
-        l_a *= ca; l_b *= cb;
-  #pragma unroll
-        for (int dt = 0; dt < 8; ++dt) { o[dt][0] *= ca; o[dt][1] *= ca; o[dt][2] *= cb; o[dt][3] *= cb; }
-        // the tensor-core fp32 accumulator truncates: a 100 s clip would chain ~600 accumulations per output.  Each
-        // 64-key block accumulates into a fresh fragment (12 MMAs deep) that is added to the running output with RN adds.
-        float oc[8][4];
-  #pragma unroll
-        for (int dt = 0; dt < 8; ++dt) oc[dt][0] = oc[dt][1] = oc[dt][2] = oc[dt][3] = 0.f;
-        // b0 = V^T[d = 8 dt + g][keys kb + 16 j2 + 2t, +1] = word ((kb + 16 j2) / 2 + t) of row d, b1 = that + 4
-  #pragma unroll
-        for (int j2 = 0; j2 < 4; ++j2) {
-          if (c0 + kb + j2 * 16 >= T) break;
-          float p[8];
-  #pragma unroll
-          for (int q = 0; q < 2; ++q) {
-            p[q * 4 + 0] = expf(sc[2 * j2 + q][0] - mn_a);
-            p[q * 4 + 1] = expf(sc[2 * j2 + q][1] - mn_a);
-            p[q * 4 + 2] = expf(sc[2 * j2 + q][2] - mn_b);
-            p[q * 4 + 3] = expf(sc[2 * j2 + q][3] - mn_b);
-          }
-          l_a += (p[0] + p[1]) + (p[4] + p[5]);
-          l_b += (p[2] + p[3]) + (p[6] + p[7]);
-          uint32_t ph[4], pl[4];
-          split_h2(p[0] * 1024.f, p[1] * 1024.f, ph[0], pl[0]);
-          split_h2(p[2] * 1024.f, p[3] * 1024.f, ph[1], pl[1]);
-          split_h2(p[4] * 1024.f, p[5] * 1024.f, ph[2], pl[2]);
-          split_h2(p[6] * 1024.f, p[7] * 1024.f, ph[3], pl[3]);
-          uint32_t bh0[8], bh1[8], bl0[8], bl1[8];
-  #pragma unroll
-          for (int dt = 0; dt < 8; ++dt) {
-            const int w = (dt * 8 + g) * VW + (kb >> 1) + j2 * 8 + t;
-            bh0[dt] = Vh[w]; bh1[dt] = Vh[w + 4]; bl0[dt] = Vl[w]; bl1[dt] = Vl[w + 4];
-          }
-  #pragma unroll
-          for (int dt = 0; dt < 8; ++dt) mma_f16(oc[dt], pl, bh0[dt], bh1[dt]);
-  #pragma unroll
-          for (int dt = 0; dt < 8; ++dt) mma_f16(oc[dt], ph, bl0[dt], bl1[dt]);
-  #pragma unroll
-          for (int dt = 0; dt < 8; ++dt) mma_f16(oc[dt], ph, bh0[dt], bh1[dt]);
-        }
-  #pragma unroll
-        for (int dt = 0; dt < 8; ++dt) { o[dt][0] += oc[dt][0]; o[dt][1] += oc[dt][1]; o[dt][2] += oc[dt][2]; o[dt][3] += oc[dt][3]; }
-      }
+      for (int kb = 0; live && kb < Tp && c0 + kb < T; kb += 64) att16_block(Kh, Kl, Vh, Vl, VW, kb, c0, T, qh, ql, o, m_a, m_b, l_a, l_b, g, t);
     }
     l_a += __shfl_xor_sync(0xffffffffu, l_a, 1);
     l_a += __shfl_xor_sync(0xffffffffu, l_a, 2);
@@ -1164,73 +1100,106 @@ static unsigned short* pack_posconv16(ts_engine* e, const float* w, float* unsca
   return e->upload(P);
 }
 
-static void attention(ts_engine* e, const float* qkv, const Act3& o, int B, int T, int H, cudaStream_t s) {
-  if (e->ws.sizing) return;
-  float* out = o.p;
-  float* out_lo = o.lo;
+// attention kernels by number (ts_debug_attention's numbering; TS_ATT_MMA 0..2 name the first three)
+enum { ATT_FFMA = 0, ATT_TF32 = 1, ATT_MMA16 = 2, ATT_MMA16P = 3, ATT_MMA16T = 4 };
+constexpr int ATT_CH = 320;                     // keys per chunk of the KV-tiled kernel in the face forward
+constexpr size_t ATT_SMEM_MAX = 220 * 1024;
+static size_t att_ffma_smem(int QT, int T) { return (size_t)(QT * 65 + 64 * 65 + QT * ((T + 63) & ~63)) * sizeof(float); }
+// query rows per CTA of the FFMA kernel: the most whose score tile fits (0: none, T > 3136)
+static int att_ffma_qt(int T) {
+  for (int QT = 64; QT >= 16; QT /= 2)
+    if (att_ffma_smem(QT, T) <= ATT_SMEM_MAX) return QT;
+  return 0;
+}
+// dynamic shared memory of attention kernel `k` for a clip of T frames (ch: keys per chunk of ATT_MMA16T); 0 when the
+// kernel cannot hold the clip
+static size_t att_smem(int k, int T, int ch) {
+  const size_t Tp = (size_t)((T + 63) & ~63);
+  size_t b;
+  switch (k) {
+    case ATT_FFMA: { const int QT = att_ffma_qt(T); return QT ? att_ffma_smem(QT, T) : 0; }
+    case ATT_TF32: b = 2 * Tp * ATT_LD * sizeof(float); break;
+    case ATT_MMA16: b = Tp * (ATT_LDK + ATT_LDV) * sizeof(float); break;
+    case ATT_MMA16P: b = (2 * Tp * ATT_KW + 2 * 64 * (Tp / 2 + 4)) * sizeof(uint32_t); break;
+    default: b = ((size_t)2 * ch * ATT_KW + (size_t)2 * 64 * (ch / 2 + 4)) * sizeof(uint32_t); break;
+  }
+  return b <= ATT_SMEM_MAX ? b : 0;
+}
+// the kernel the face forward runs for a clip of T frames: TS_ATT_MMA picks the family, the clip length the member
+static int att_kernel_for(int T) {
   static const int att_mode = getenv("TS_ATT_MMA") ? atoi(getenv("TS_ATT_MMA")) : 3;   // A/B switch: 0 FFMA, 1 tf32 MMA, 2 fp16-split MMA, 3 fp16-split MMA with K/V split once per CTA
-  if (att_mode == 3) {
-    const int Tp64 = (T + 63) & ~63;
-    const size_t smem16p = ((size_t)2 * Tp64 * ATT_KW + (size_t)2 * 64 * (Tp64 / 2 + 4)) * sizeof(uint32_t);
-    if (smem16p <= 220 * 1024) {
-      TS_CUDA(cudaFuncSetAttribute(attention_mma16p_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem16p));
-      attention_mma16p_kernel<<<B * H, ATT_WARPS * 32, smem16p, s>>>(qkv, out, out_lo, o.h16, o.l16, T, H, 0.125f);
-      e->launches++;
-      TS_CUDA(cudaGetLastError());
-      return;
+  if (att_mode == 3) return att_smem(ATT_MMA16P, T, 0) ? ATT_MMA16P : ATT_MMA16T;   // longer than 12.8 s: keys / values staged in chunks
+  if (att_mode == 2 && att_smem(ATT_MMA16, T, 0)) return ATT_MMA16;
+  if (att_mode != 0 && att_smem(ATT_TF32, T, 0)) return ATT_TF32;
+  return ATT_FFMA;
+}
+
+// o = softmax(q k^T / 8) v per head on kernel `kernel` (ch: keys per chunk of ATT_MMA16T), into o's format: plain fp32,
+// 3xTF32 (hi, lo) pair, or fp32 with fp16 planes (ATT_MMA16P / ATT_MMA16T only)
+static void attention(ts_engine* e, int kernel, int ch, const float* qkv, const Act3& o, int B, int T, int H, cudaStream_t s) {
+  if (e->ws.sizing) return;
+  const size_t smem = att_smem(kernel, T, ch);
+  if (!smem) fail(TS_ERR_UNSUPPORTED, "attention: %d frames exceed the shared memory of kernel %d", T, kernel);
+  if (o.h16 && kernel < ATT_MMA16P)
+    fail(TS_ERR_UNSUPPORTED, "attention: kernel %d has no fp16-split output (use the default, or ts_set_tensor_cores(e, 1))", kernel);
+  const float scale = 0.125f;  // head_dim ** -0.5
+  auto smem_attr = [&](const void* fn) { TS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); };
+  switch (kernel) {
+    case ATT_MMA16P:
+      smem_attr((const void*)attention_mma16p_kernel);
+      attention_mma16p_kernel<<<B * H, ATT_WARPS * 32, smem, s>>>(qkv, o.p, o.lo, o.h16, o.l16, T, H, scale);
+      break;
+    case ATT_MMA16T:
+      smem_attr((const void*)attention_mma16t_kernel);
+      attention_mma16t_kernel<<<dim3(B * H, cdiv(cdiv(T, 16), ATT_WARPS)), ATT_WARPS * 32, smem, s>>>(qkv, o.p, o.lo, o.h16, o.l16, T, H, scale, ch);
+      break;
+    case ATT_MMA16:
+      smem_attr((const void*)attention_mma16_kernel);
+      attention_mma16_kernel<<<B * H, ATT_WARPS * 32, smem, s>>>(qkv, o.p, o.lo, T, H, scale);
+      break;
+    case ATT_TF32:
+      smem_attr((const void*)attention_mma_kernel);
+      attention_mma_kernel<<<B * H, ATT_WARPS * 32, smem, s>>>(qkv, o.p, o.lo, T, H, scale);
+      break;
+    default: {
+      const int QT = att_ffma_qt(T);
+      if (QT == 64) {
+        smem_attr((const void*)attention_kernel<64>);
+        attention_kernel<64><<<dim3(cdiv(T, 64), B * H), 256, smem, s>>>(qkv, o.p, o.lo, T, H, scale);
+      } else if (QT == 32) {
+        smem_attr((const void*)attention_kernel<32>);
+        attention_kernel<32><<<dim3(cdiv(T, 32), B * H), 256, smem, s>>>(qkv, o.p, o.lo, T, H, scale);
+      } else {
+        smem_attr((const void*)attention_kernel<16>);
+        attention_kernel<16><<<dim3(cdiv(T, 16), B * H), 256, smem, s>>>(qkv, o.p, o.lo, T, H, scale);
+      }
     }
-    // longer than 12.8 s: the same arithmetic, keys / values staged 320 at a time (no length limit)
-    const int CH = 320;
-    const size_t smem16t = ((size_t)2 * CH * ATT_KW + (size_t)2 * 64 * (CH / 2 + 4)) * sizeof(uint32_t);
-    TS_CUDA(cudaFuncSetAttribute(attention_mma16t_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem16t));
-    const int nrb = (T + 15) / 16;
-    attention_mma16t_kernel<<<dim3(B * H, cdiv(nrb, ATT_WARPS)), ATT_WARPS * 32, smem16t, s>>>(qkv, out, out_lo, o.h16, o.l16, T, H, 0.125f, CH);
+  }
+  e->launches++;
+  TS_CUDA(cudaGetLastError());
+}
+
+// positional conv embedding (Conv1d 768 -> 768, k = 128, groups = 16, pad 64, last output dropped) + GELU: x [B,T,768] with
+// 64 zero pad rows -> y [B,T,768].  posconv_mma_kernel on the pre-split weights when the tensor cores are on, else the FFMA
+// GEMM with one grid z-slice per group on the packed Layer.
+static void posconv(ts_engine* e, const Layer& L, const unsigned short* w16, float unscale, const Act3& x, const Act3& y, cudaStream_t s) {
+  if (e->ws.sizing) return;
+  if (x.pad != 64 || x.C != 768 || y.C != 768 || y.T != x.T || y.B != x.B) fail(TS_ERR_INVALID, "posconv: activation geometry");
+  const int B = x.B, T = x.T;
+  if (e->use_tc && w16) {
+    TS_CUDA(cudaFuncSetAttribute(posconv_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PC_SMEM));
+    posconv_mma_kernel<<<dim3(B * 16, cdiv(T, PC_ROWS)), PC_WARPS * 32, PC_SMEM, s>>>(x, w16, L.bias, unscale, y);
     e->launches++;
     TS_CUDA(cudaGetLastError());
     return;
   }
-  if (o.h16) fail(TS_ERR_UNSUPPORTED, "attention: TS_ATT_MMA=%d has no fp16-split output (use the default, or ts_set_tensor_cores(e, 1))", att_mode);
-  if (att_mode == 2 || att_mode == 3) {
-    const int Tp64 = (T + 63) & ~63;
-    const size_t smem16 = (size_t)Tp64 * (ATT_LDK + ATT_LDV) * sizeof(float);
-    if (smem16 <= 220 * 1024) {
-      TS_CUDA(cudaFuncSetAttribute(attention_mma16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem16));
-      attention_mma16_kernel<<<B * H, ATT_WARPS * 32, smem16, s>>>(qkv, out, out_lo, T, H, 0.125f);
-      e->launches++;
-      TS_CUDA(cudaGetLastError());
-      return;
-    }
-  }
-  {
-    const bool use_mma = att_mode != 0;
-    const int Tp64 = (T + 63) & ~63;
-    const size_t smem_mma = (size_t)2 * Tp64 * ATT_LD * sizeof(float);
-    if (use_mma && smem_mma <= 220 * 1024) {
-      TS_CUDA(cudaFuncSetAttribute(attention_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_mma));
-      attention_mma_kernel<<<B * H, ATT_WARPS * 32, smem_mma, s>>>(qkv, out, out_lo, T, H, 0.125f);
-      e->launches++;
-      TS_CUDA(cudaGetLastError());
-      return;
-    }
-  }
-  const int Tp = (T + 63) & ~63;
-  auto smem = [&](int QT) { return (size_t)(QT * 65 + 64 * 65 + QT * Tp) * sizeof(float); };
-  const float scale = 0.125f;  // head_dim ** -0.5
-  const size_t lim = 220 * 1024;
-  if (smem(64) <= lim) {
-    TS_CUDA(cudaFuncSetAttribute(attention_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem(64)));
-    attention_kernel<64><<<dim3(cdiv(T, 64), B * H), 256, smem(64), s>>>(qkv, out, out_lo, T, H, scale);
-  } else if (smem(32) <= lim) {
-    TS_CUDA(cudaFuncSetAttribute(attention_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem(32)));
-    attention_kernel<32><<<dim3(cdiv(T, 32), B * H), 256, smem(32), s>>>(qkv, out, out_lo, T, H, scale);
-  } else if (smem(16) <= lim) {
-    TS_CUDA(cudaFuncSetAttribute(attention_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem(16)));
-    attention_kernel<16><<<dim3(cdiv(T, 16), B * H), 256, smem(16), s>>>(qkv, out, out_lo, T, H, scale);
-  } else {
-    fail(TS_ERR_UNSUPPORTED, "attention: %d frames exceed the shared-memory score tile (max ~3000 frames = 100 s)", T);
-  }
-  e->launches++;
-  TS_CUDA(cudaGetLastError());
+  GemmP p;
+  p.A = x.row(0, -64); p.W = L.W; p.bias = L.bias; p.C = y.row(0, 0);
+  p.M = B * T; p.N = 48; p.K = 128 * 48; p.mper = T;
+  p.a_bs = x.bstride(); p.a_rs = 768; p.kc = 48; p.a_ts = 768;
+  p.c_bs = y.bstride(); p.c_rs = 768; p.act = ACT_GELU; p.ldw = 128 * 48;
+  p.groups = 16; p.a_goff = 48; p.w_goff = (long)48 * 128 * 48; p.n_goff = 48;
+  launch_gemm(e, p, s);
 }
 
 // Linear on channel-last activations: y[:, coff:coff+N] = act(x W^T + b (+ res)) — a 1-tap conv
@@ -1276,22 +1245,7 @@ void face_run(ts_engine* e, const float* wave, const float* idv, float* out, int
   linear(e, F.fproj, hn, x, ACT_NONE, nullptr, s);
   // ---- positional conv embedding (k=128, groups=16, pad 64, last output dropped) + LN -----------
   Act3 pc = new_act(e, B, frame, 768, 0, s);
-  if (e->use_tc && F.pos_w16) {
-    if (!e->ws.sizing) {
-      TS_CUDA(cudaFuncSetAttribute(posconv_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PC_SMEM));
-      posconv_mma_kernel<<<dim3(B * 16, cdiv(frame, PC_ROWS)), PC_WARPS * 32, PC_SMEM, s>>>(x, F.pos_w16, F.posconv.bias, F.pos_unscale, pc);
-      e->launches++;
-      TS_CUDA(cudaGetLastError());
-    }
-  } else {
-    GemmP p;
-    p.A = x.row(0, -64); p.W = F.posconv.W; p.bias = F.posconv.bias; p.C = pc.row(0, 0);
-    p.M = B * frame; p.N = 48; p.K = 128 * 48; p.mper = frame;
-    p.a_bs = x.bstride(); p.a_rs = 768; p.kc = 48; p.a_ts = 768;
-    p.c_bs = pc.bstride(); p.c_rs = 768; p.act = ACT_GELU; p.ldw = 128 * 48;
-    p.groups = 16; p.a_goff = 48; p.w_goff = (long)48 * 128 * 48; p.n_goff = 48;
-    launch_gemm(e, p, s);
-  }
+  posconv(e, F.posconv, F.pos_w16, F.pos_unscale, x, pc, s);
   Act3 hcur = new_act(e, B, frame, 768, 0, s, tc);
   ln_pre(e, x, &pc, F.enc_ln_g, F.enc_ln_b, hcur, nullptr, ACT_NONE, s);
   // ---- 12 post-LN transformer layers ------------------------------------------------------------
@@ -1301,7 +1255,7 @@ void face_run(ts_engine* e, const float* wave, const float* idv, float* out, int
   Act3 ff = new_act(e, B, frame, 3072, 0, s, tc);
   for (auto& L : F.layers) {
     linear(e, L.qkv, hcur, qkv, ACT_NONE, nullptr, s);
-    attention(e, qkv.p, att, B, frame, 12, s);
+    attention(e, att_kernel_for(frame), ATT_CH, qkv.p, att, B, frame, 12, s);
     linear(e, L.out, att, t1, ACT_NONE, &hcur, s);                       // h + out_proj(attn)
     ln_pre(e, t1, nullptr, L.ln1_g, L.ln1_b, hcur, nullptr, ACT_NONE, s);
     linear(e, L.ff1, hcur, ff, ACT_GELU, nullptr, s);
@@ -1466,3 +1420,72 @@ extern "C" int ts_face_forward(ts_engine* e, const float* wave, const float* id,
 }
 
 extern "C" int ts_face_dim(ts_engine* e) { return (e && e->face) ? e->face->jaw_dim + e->face->exp_dim : 0; }
+
+extern "C" int ts_debug_attention(ts_engine* e, const ts_debug_att* a, const float* qkv, float* out, void* plane_hi, void* plane_lo,
+                                  void* stream) {
+  TS_API_BEGIN(e)
+  require_device(e);
+  if (!a || !qkv) fail(TS_ERR_INVALID, "ts_debug_attention: a and qkv are required");
+  const ts_debug_att g = *a;
+  const int H = 12;
+  if (g.B < 1 || g.T < 1) fail(TS_ERR_INVALID, "ts_debug_attention: B %d, T %d (need >= 1)", g.B, g.T);
+  if ((long)g.B * g.T > INT_MAX / (3 * H * 64)) fail(TS_ERR_INVALID, "ts_debug_attention: more than 2^31 - 1 qkv elements");
+  if (g.kernel < -1 || g.kernel > ATT_MMA16T)
+    fail(TS_ERR_INVALID, "ts_debug_attention: kernel %d (-1 the face forward's choice, 0 FFMA, 1 tf32, 2 mma16, 3 mma16p, 4 mma16t)", g.kernel);
+  if (g.out_format < 0 || g.out_format > 2)
+    fail(TS_ERR_INVALID, "ts_debug_attention: out_format %d (0 fp32, 1 fp32 hi / lo, 2 fp32 + fp16 planes)", g.out_format);
+  const int kernel = g.kernel < 0 ? att_kernel_for(g.T) : g.kernel;
+  if (g.chunk && (kernel != ATT_MMA16T || g.chunk % 64 || g.chunk < 64 || g.chunk > 384))
+    fail(TS_ERR_INVALID, "ts_debug_attention: chunk %d (kernel 4 only: a multiple of 64 in [64, 384])", g.chunk);
+  const int ch = g.chunk ? g.chunk : ATT_CH;
+  if (!att_smem(kernel, g.T, ch)) fail(TS_ERR_INVALID, "ts_debug_attention: kernel %d cannot hold %d frames in shared memory", kernel, g.T);
+  if (g.out_format == 2 && kernel < ATT_MMA16P) fail(TS_ERR_INVALID, "ts_debug_attention: kernel %d has no fp16-split output", kernel);
+  if ((g.out_format != 1 && !out) || (g.out_format != 0 && (!plane_hi || !plane_lo)))
+    fail(TS_ERR_INVALID, "ts_debug_attention: out_format %d needs %s", g.out_format,
+         g.out_format == 0 ? "out" : g.out_format == 1 ? "plane_hi and plane_lo" : "out, plane_hi and plane_lo");
+
+  TcModeGuard guard(e, g.out_format == 0 ? 0 : g.out_format == 1 ? 1 : 6);   // the activation format face_run gives `att`
+  cudaStream_t s = (cudaStream_t)stream;
+  const size_t nq = (size_t)g.B * g.T * 3 * H * 64, nguard = (size_t)64 * 3 * H * 64;
+  float* q = nullptr;
+  Act3 o;
+  run_sized(e, [&] {
+    q = e->ws.alloc<float>(nq + nguard);
+    o = new_act(e, g.B, g.T, H * 64, 0, s, g.out_format != 0);
+  });
+  TS_CUDA(cudaMemcpyAsync(q, qkv, nq * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  TS_CUDA(cudaMemsetAsync(q + nq, 0xff, nguard * sizeof(float), s));   // 64 NaN rows after the last item: no kernel may read them
+  debug_planes(o, out, plane_hi, plane_lo, false, s);
+  attention(e, kernel, ch, q, o, g.B, g.T, H, s);
+  debug_planes(o, out, plane_hi, plane_lo, true, s);
+  TS_CUDA(cudaStreamSynchronize(s));
+  TS_API_END(e)
+}
+
+extern "C" int ts_debug_posconv(ts_engine* e, int mode, const float* x, const float* W_host, const float* bias_host, float* y, int B, int T,
+                                void* stream) {
+  TS_API_BEGIN(e)
+  require_device(e);
+  if (!x || !W_host || !bias_host || !y) fail(TS_ERR_INVALID, "ts_debug_posconv: x, W_host, bias_host and y are required");
+  if (mode != 0 && mode != 1 && mode != 6) fail(TS_ERR_INVALID, "ts_debug_posconv: mode %d (0 FFMA grouped GEMM, 1 / 6 HMMA kernel)", mode);
+  if (B < 1 || T < 1) fail(TS_ERR_INVALID, "ts_debug_posconv: B %d, T %d (need >= 1)", B, T);
+  if ((long)B * (T + 128) > INT_MAX / 768) fail(TS_ERR_INVALID, "ts_debug_posconv: more than 2^31 - 1 activation elements");
+  LoadScope scope(e, "debug_posconv");   // this call's weights replace the previous call's
+  const Layer L = pack_ckc(e, W_host, bias_host, 768, 48, 128);
+  float unscale = 1.f;
+  const unsigned short* w16 = pack_posconv16(e, W_host, &unscale);
+  TcModeGuard guard(e, mode);
+  cudaStream_t s = (cudaStream_t)stream;
+  Act3 xa, ya;
+  run_sized(e, [&] {
+    xa = new_act(e, B, T, 768, 64, s);   // face_run's x: 64 zero pad rows around every item
+    ya = new_act(e, B, T, 768, 0, s);
+  });
+  debug_fill(e, x, xa, s);
+  debug_planes(ya, y, nullptr, nullptr, false, s);
+  posconv(e, L, w16, unscale, xa, ya, s);
+  debug_planes(ya, y, nullptr, nullptr, true, s);
+  TS_CUDA(cudaStreamSynchronize(s));
+  scope.commit();
+  TS_API_END(e)
+}

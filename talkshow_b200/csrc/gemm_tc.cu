@@ -528,19 +528,19 @@ __global__ void debug_fill_kernel(const float* __restrict__ x, Act3 a) {
   }
 }
 
-// The engine's dense-kernel switches for one call, restored however the call ends
-struct TcModeGuard {
-  ts_engine* e;
-  bool use_tc, tc_f16;
-  TcModeGuard(ts_engine* e_, int mode) : e(e_), use_tc(e_->use_tc), tc_f16(e_->tc_f16) {
-    e->use_tc = mode != 0;
-    e->tc_f16 = mode == 6;
-  }
-  ~TcModeGuard() {
-    e->use_tc = use_tc;
-    e->tc_f16 = tc_f16;
-  }
-};
+void debug_fill(ts_engine* e, const float* x, const Act3& a, cudaStream_t s) {
+  debug_fill_kernel<<<(int)std::min<long>((long)(a.numel() + 255) / 256, (long)e->sm_count * 16), 256, 0, s>>>(x, a);
+  e->launches++;
+  TS_CUDA(cudaGetLastError());
+}
+
+void debug_planes(const Act3& a, float* y, void* plane_hi, void* plane_lo, bool back, cudaStream_t s) {
+  const size_t n = a.numel();
+  struct Plane { void* dev; void* user; size_t bytes; };
+  const Plane planes[4] = {{a.p, a.lo ? plane_hi : (void*)y, n * 4}, {a.lo, plane_lo, n * 4}, {a.h16, plane_hi, n * 2}, {a.l16, plane_lo, n * 2}};
+  for (const Plane& p : planes)
+    if (p.dev) TS_CUDA(cudaMemcpyAsync(back ? p.user : p.dev, back ? p.dev : p.user, p.bytes, cudaMemcpyDeviceToDevice, s));
+}
 }  // namespace ts
 
 extern "C" int ts_debug_conv1d(ts_engine* e, const ts_debug_conv* a, const float* x, const float* W_host, const float* bias_host,
@@ -602,24 +602,12 @@ extern "C" int ts_debug_conv1d(ts_engine* e, const ts_debug_conv* a, const float
     ya = new_act(e, g.B, g.y_T, g.y_C, g.y_pad, s, g.y_split != 0, 0, y_planes);
     if (res) ra = new_act(e, g.B, g.T_out, g.N, g.res_pad, s, g.res_split != 0);
   });
-  auto fill = [&](const float* src, const Act3& dst) {
-    debug_fill_kernel<<<(int)std::min<long>((long)(dst.numel() + 255) / 256, (long)e->sm_count * 16), 256, 0, s>>>(src, dst);
-    e->launches++;
-    TS_CUDA(cudaGetLastError());
-  };
-  fill(x, xa);
-  if (res) fill(res, ra);
-  // y's planes: hi / lo fp32 (modes 0, 1: ya.p is the hi plane) or h16 / l16 (mode 6)
-  const size_t yn = ya.numel();
-  struct Plane { void* dev; void* user; size_t bytes; };
-  const Plane planes[4] = {{ya.p, ya.lo ? y_plane_hi : (void*)y, yn * 4}, {ya.lo, y_plane_lo, yn * 4},
-                           {ya.h16, y_plane_hi, yn * 2}, {ya.l16, y_plane_lo, yn * 2}};
-  for (const Plane& p : planes)
-    if (p.dev) TS_CUDA(cudaMemcpyAsync(p.dev, p.user, p.bytes, cudaMemcpyDeviceToDevice, s));
+  debug_fill(e, x, xa, s);
+  if (res) debug_fill(e, res, ra, s);
+  debug_planes(ya, y, y_plane_hi, y_plane_lo, false, s);
   if (mode == 0) conv1d(e, L, xa, g.k, g.stride, g.pd, ya, g.T_out, g.act, res ? &ra : nullptr, s, g.y_tmul, g.y_toff, 0, g.coff);
   else tc_conv1d(e, L, xa, g.k, g.stride, g.pd, ya, g.T_out, g.act, res ? &ra : nullptr, s, g.y_tmul, g.y_toff, g.coff, g.chunk);
-  for (const Plane& p : planes)
-    if (p.dev) TS_CUDA(cudaMemcpyAsync(p.user, p.dev, p.bytes, cudaMemcpyDeviceToDevice, s));
+  debug_planes(ya, y, y_plane_hi, y_plane_lo, true, s);
   TS_CUDA(cudaStreamSynchronize(s));
   scope.commit();
   TS_API_END(e)

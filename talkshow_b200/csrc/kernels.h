@@ -93,6 +93,27 @@ void upload_weights(ts_engine* e, const std::vector<float>& W, Layer* L);
 void conv_auto(ts_engine* e, const Layer& L, const Act3& x, int k, int stride, int pd, const Act3& y, int T_out, int act,
                const Act3* res, cudaStream_t s, int y_tmul = 1, int y_toff = 0, int coff = 0);
 
+// ---- debug entry points (ts_debug_*): one kernel on caller data, staged as the nets stage it ----------------------------
+// x [B, a.T, a.C] -> rows [0, a.T) of every item of `a`, in a's storage format (fp32, 3xTF32 pair or fp32 + fp16 planes);
+// the tail rows of every plane get NaN (no kernel may read them), pad rows keep new_act's zeros
+void debug_fill(ts_engine* e, const float* x, const Act3& a, cudaStream_t s);
+// copy the caller's output buffers into a's planes (back = false) or a's planes out to them (back = true): y <-> a.p, or
+// plane_hi / plane_lo <-> the (hi, lo) pair (a.p, a.lo) or the fp16 planes (a.h16, a.l16) beside y <-> a.p
+void debug_planes(const Act3& a, float* y, void* plane_hi, void* plane_lo, bool back, cudaStream_t s);
+// the engine's dense-kernel switches (ts_set_tensor_cores numbering) for one call, restored however the call ends
+struct TcModeGuard {
+  ts_engine* e;
+  bool use_tc, tc_f16;
+  TcModeGuard(ts_engine* e_, int mode) : e(e_), use_tc(e_->use_tc), tc_f16(e_->tc_f16) {
+    e->use_tc = mode != 0;
+    e->tc_f16 = mode == 6;
+  }
+  ~TcModeGuard() {
+    e->use_tc = use_tc;
+    e->tc_f16 = tc_f16;
+  }
+};
+
 #ifdef __CUDACC__
 // two-term fp16 split of an fp32 value: h = fp16(x), l = fp16(x - h) (22 significant bits while l stays normal)
 __device__ __forceinline__ void split16(float x, unsigned short& h, unsigned short& l) {
