@@ -136,6 +136,30 @@ typedef struct ts_sample_ctl {
 int ts_pixelcnn_sample_ctl(ts_engine* e, const float* aud, const int64_t* label, const float* noise, int64_t* idx_out,
                            float* logits_out, int B, int T, const int64_t* pre_latents, int T0,
                            const ts_sample_ctl* ctl, void* stream);
+/* ---- seeded sampling: per-clip counter-based noise generated inside the sampler --------------------------------------
+ * RNG contract.  The draw at absolute latent row r (rows forced by pre_latents count: a call with T0 prefix rows samples
+ * rows T0 .. T0+T-1), column c in {0,1}, code n in [0,2048), of a clip with seed s (int64, used as its 64 bits) divides by
+ *     x = Philox4x32-10(counter = (n & 511, r, c, 0), key = (s & 0xffffffff, s >> 32))[n >> 9]
+ *     u = (float)((x >> 8) | 1) * 2^-24        an odd multiple of 2^-24: exact in fp32, in [2^-24, 1 - 2^-24]
+ *     q = -logf(u)                             > 0, never inf
+ * Philox4x32-10 is the Random123 / cuRAND generator (multipliers 0xD2511F53, 0xCD9E8D57; key increments 0x9E3779B9,
+ * 0xBB67AE85).  A clip's noise depends only on its seed and the absolute position of the draw: not on B, T, the clip's
+ * place in the batch, the executor or how the clip is split into chunks.  The draw itself (argmax(p / q), every
+ * sampling control) is unchanged.
+ *
+ * The Exp(1) values of the seeded sampler in the layout of `noise` of ts_pixelcnn_generate: seeds [B] (device),
+ * noise_out [2T,B,2048], block 2(r-T0)+c holds row r in [T0, T0+T).  One launch.  TS_ERR_INVALID: B, T <= 0, T0 < 0,
+ * 2TB >= 2^31, NULL seeds or noise_out. */
+int ts_sampler_noise(ts_engine* e, const int64_t* seeds, float* noise_out, int B, int T, int T0, void* stream);
+/* ts_pixelcnn_sample_ctl with seeds [B] (device, int64) in place of noise: there is no noise tensor.  ctl may be NULL: the
+ * default draw of ts_pixelcnn_generate.  Equivalences: with ctl, the call equals ts_pixelcnn_sample_ctl(noise =
+ * ts_sampler_noise(seeds, B, T, T0)) bit for bit (codes, logits_out, logp_out, kept_out); with ctl = NULL it equals
+ * ts_pixelcnn_generate on that noise.  The launches are those of ts_pixelcnn_generate (no extra kernel, no noise buffer).
+ * seeds may be NULL only for greedy decoding (ctl->temperature = 0); otherwise TS_ERR_INVALID, like the conditions of
+ * ts_pixelcnn_sample_ctl. */
+int ts_pixelcnn_sample_seeded(ts_engine* e, const float* aud, const int64_t* label, const int64_t* seeds, int64_t* idx_out,
+                              float* logits_out, int B, int T, const int64_t* pre_latents, int T0,
+                              const ts_sample_ctl* ctl, void* stream);
 /* GatedPixelCNN.forward (teacher forced), :130-150, for rows [0,T): logits_out [B,2048,T,2]. */
 int ts_pixelcnn_logits(ts_engine* e, const float* aud, const int64_t* label, const int64_t* codes,
                        float* logits_out, int B, int T, void* stream);
@@ -203,6 +227,11 @@ int ts_body_sample(ts_engine* e, const float* mfcc, const int64_t* label, const 
  * ts_body_sample is this call with top_p = 1, min_p = 0 and kept_out = NULL. */
 int ts_body_sample_ctl(ts_engine* e, const float* mfcc, const int64_t* label, const float* noise, int64_t* codes,
                        float* poses, int B, int M, const ts_sample_ctl* ctl, void* stream);
+/* ts_body_sample_ctl with seeds [B] (device) in place of noise, the RNG contract of ts_pixelcnn_sample_seeded; ctl may be
+ * NULL (the default draw of ts_body_generate).  Same launches as ts_body_generate; seeds may be NULL only for greedy
+ * decoding (TS_ERR_INVALID otherwise). */
+int ts_body_sample_seeded(ts_engine* e, const float* mfcc, const int64_t* label, const int64_t* seeds, int64_t* codes,
+                          float* poses, int B, int M, const ts_sample_ctl* ctl, void* stream);
 
 /* Audio front-end of get_mfcc_ta, data_utils/utils.py:148-177 (SURVEY.md §8f-1): wave [B,N] mono at
  * `sr` Hz -> torchaudio Resample(sr, 22000) -> MFCC(64 coefficients, n_fft 2048, hop 734 = 30 fps, 256 HTK

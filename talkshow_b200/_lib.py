@@ -55,6 +55,11 @@ SYMBOLS = {
                                          C.c_int, C.c_int, C.c_void_p, C.c_int, C.POINTER(ts_sample_ctl), C.c_void_p]),
     "ts_body_sample_ctl": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                      C.c_int, C.POINTER(ts_sample_ctl), C.c_void_p]),
+    "ts_sampler_noise": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "ts_pixelcnn_sample_seeded": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_int, C.c_int, C.c_void_p, C.c_int, C.POINTER(ts_sample_ctl), C.c_void_p]),
+    "ts_body_sample_seeded": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                        C.c_int, C.POINTER(ts_sample_ctl), C.c_void_p]),
     "ts_pixelcnn_logits": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                      C.c_void_p]),
     "ts_pixelcnn_score": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,

@@ -471,6 +471,8 @@ struct PixArgs {
   float* logp_out;     // [B][Ttot-T0][2] or null
   float top_p, min_p;
   int* kept_out;       // [B][Ttot-T0][2] or null
+  // seeded sampling (ts_pixelcnn_sample_seeded): [B] per-clip seeds; the draw's q comes from seeded_q, noise is unread
+  const int64_t* seeds;
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -1271,10 +1273,56 @@ __device__ __forceinline__ long long draw_controlled(const float (&l)[8], const 
   return code;
 }
 
+// ---- seeded noise: the RNG contract of ts_pixelcnn_sample_seeded (include/talkshow_b200.h) --------------------------
+// Philox4x32-10 (Salmon et al., SC'11; the Random123 / cuRAND generator), the ten rounds written out.
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
+#pragma unroll
+  for (int i = 0; i < 10; ++i) {
+    const uint32_t lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
+    const uint32_t lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
+    c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+    k0 += 0x9E3779B9u;
+    k1 += 0xBB67AE85u;
+  }
+  return c;
+}
+
+// Exp(1) value of one 32-bit output: u = ((x >> 8) | 1) 2^-24 is an odd multiple of 2^-24 (exact in fp32, never 0 or 1),
+// so q = -log(u) lies in (0, 16.7] and is never inf
+__device__ __forceinline__ float philox_exp1(uint32_t x) { return -logf((float)((x >> 8) | 1u) * 0x1p-24f); }
+
+// The q of codes tid + 256 j (j = 0..7) of draw (absolute latent row r, column c) of the clip seeded `seed`: code n is
+// output n >> 9 of counter (n & 511, r, c, 0) under key (seed lo, seed hi), so the thread evaluates counters tid and
+// tid + 256 and uses all four outputs of each.  One definition for both executors and ts_sampler_noise.
+__device__ __forceinline__ void seeded_q(int64_t seed, int r, int c, int tid, float (&q)[8]) {
+  const uint32_t k0 = (uint32_t)(uint64_t)seed, k1 = (uint32_t)((uint64_t)seed >> 32);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const uint4 x = philox4x32_10(make_uint4((uint32_t)(tid + 256 * h), (uint32_t)r, (uint32_t)c, 0u), k0, k1);
+    q[h] = philox_exp1(x.x);
+    q[2 + h] = philox_exp1(x.y);
+    q[4 + h] = philox_exp1(x.z);
+    q[6 + h] = philox_exp1(x.w);
+  }
+}
+
+// The noise of draw (r, c) of sample m (global clip index): computed from A.seeds, else read from A.noise.
+template <class Args>
+__device__ __forceinline__ void draw_noise(const Args& A, int r, int c, int m, float (&q)[8]) {
+  const int tid = threadIdx.x;
+  if (A.seeds) {
+    seeded_q(A.seeds[m], r, c, tid, q);
+  } else {
+    const float* src = A.noise + ((size_t)(2 * (r - A.T0) + c) * A.B + m) * PIX_NCODE;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) q[j] = __ldcs(src + tid + 256 * j);
+  }
+}
+
 // softmax over 2048 logits + categorical draw = argmax(p / q) (ATen multinomial, num_samples = 1),
 // then embedding gather of the sampled code into the E ring.  One CTA per sample.
-// QPRE (persistent kernel): the sampler noise of this position was loaded before the grid-barrier wait (it is an
-// input of the call, independent of every stage) and arrives in qpre[8].
+// QPRE (persistent kernel): the sampler noise of this position was loaded (or, seeded, computed) before the grid-barrier
+// wait (it is an input of the call, independent of every stage) and arrives in qpre[8].  Otherwise draw_noise here.
 // WARP: the draw applies the sampling controls of A (draw_controlled); otherwise the default draw below.
 template <int MB, bool QPRE = false, bool WARP = false>
 __device__ void run_sample_task(const PixTask& t, const PixArgs& A, int r, int m, float* red, const float* qpre = nullptr) {
@@ -1301,9 +1349,12 @@ __device__ void run_sample_task(const PixTask& t, const PixArgs& A, int r, int m
     if (!forced) {
       float qv[8];
       if (A.temperature > 0.f) {
-        const float* q = A.noise + ((size_t)(2 * (r - A.T0) + c) * A.B + m) * PIX_NCODE;
+        if (QPRE) {
 #pragma unroll
-        for (int j = 0; j < 8; ++j) qv[j] = QPRE ? qpre[j] : q[tid + 256 * j];
+          for (int j = 0; j < 8; ++j) qv[j] = qpre[j];
+        } else {
+          draw_noise(A, r, c, m, qv);
+        }
       }
       const size_t at = ((size_t)m * (A.Ttot - A.T0) + (r - A.T0)) * 2 + c;
       code = draw_controlled(l, qv, A.temperature, A.top_k, A.top_p, A.min_p, red, A.logp_out ? A.logp_out + at : nullptr,
@@ -1332,13 +1383,19 @@ __device__ void run_sample_task(const PixTask& t, const PixArgs& A, int r, int m
 #pragma unroll
     for (int w = 1; w < 8; ++w) sum += sf[w];
     __syncthreads();
-    const float* q = A.noise + ((size_t)(2 * (r - A.T0) + c) * A.B + m) * PIX_NCODE;
+    float qv[8];
+    if (QPRE) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) qv[j] = qpre[j];
+    } else {
+      draw_noise(A, r, c, m, qv);
+    }
     float bv = -INFINITY;
     int bi = 0x7fffffff;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       int n = tid + 256 * j;
-      float v = (ex[j] / sum) / (QPRE ? qpre[j] : q[n]);
+      float v = (ex[j] / sum) / qv[j];
       if (v > bv || (v == bv && n < bi)) { bv = v; bi = n; }
     }
     for (int o = 16; o > 0; o >>= 1) {
@@ -1446,12 +1503,11 @@ __global__ void __launch_bounds__(PIX_THREADS, 1) pixelcnn_kernel(PixArgs A, int
     EpiPre pre;
     pre.a = pre.b = 0.f; pre.valid = false;
     if (active && t.epi != EPI_SAMPLE) pre = prefetch_epilogue<MB, S2>(t, A, r);   // in flight while we wait below
-    float qpre[8];   // the sampler noise of this position is an input of the call: in flight while we wait at the barrier
-    if (active && t.epi == EPI_SAMPLE && cta < A.B && r >= A.T0 && (!WARP || A.temperature > 0.f)) {   // greedy: no noise
-      const float* q = A.noise + ((size_t)(2 * (r - A.T0) + t.col) * A.B + cta) * PIX_NCODE;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) qpre[j] = __ldcs(q + tid + 256 * j);
-    }
+    // the sampler noise of this position is an input of the call (or, seeded, a function of the seed and the position):
+    // loaded / computed before the barrier wait, so it overlaps the wait
+    float qpre[8];
+    if (active && t.epi == EPI_SAMPLE && cta < A.B && r >= A.T0 && (!WARP || A.temperature > 0.f))   // greedy: no noise
+      draw_noise(A, r, t.col, cta, qpre);
     if (has_w) { mbar_wait(&bars[buf], uses[buf] & 1u); uses[buf]++; }
     unsigned long long* tr = nullptr;
     if constexpr (TRACE) {
@@ -1519,7 +1575,7 @@ __global__ void logits_to_ref_kernel(const float* __restrict__ in, float* __rest
 
 static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t* label, const float* noise, int noise_B,
                            int64_t* idx_out, float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s,
-                           bool logits_all, const SampleCtl* ctl) {
+                           bool logits_all, const SampleCtl* ctl, const int64_t* seeds) {
   PixelPlan* P = e->pix;
   Plan3* Q = (Plan3*)P->p3;
   const int Ttot = T0 + T, D = P->D;
@@ -1546,7 +1602,7 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
   (void)noise_B;
 
   if (v3) {   // cluster-resident executor (pixelcnn3.inc): any batch size, clusters of 16 CTAs per 4 / 8 samples
-    launch_pixelcnn3(e, P, Q, audv, audh, label, noise, idx_out, logits_out, B, T0, Ttot, pre, logits_all, arena3, MB3, s, ctl);
+    launch_pixelcnn3(e, P, Q, audv, audh, label, noise, idx_out, logits_out, B, T0, Ttot, pre, logits_all, arena3, MB3, s, ctl, seeds);
     return;
   }
   if (B > PIX_MB)
@@ -1577,6 +1633,7 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
   const SampleCtl c = ctl ? *ctl : SampleCtl();
   A.temperature = c.temperature; A.top_k = c.top_k; A.logp_out = c.logp_out;
   A.top_p = c.top_p; A.min_p = c.min_p; A.kept_out = c.kept_out;
+  A.seeds = seeds;
   if (e->pixel_mode == 0) {
     // A/B switch: 0 = burst loads + scalar FFMA, 4 = pipelined loads + scalar FFMA, 5 (default) = pipelined loads + paired FMAs (fma2)
     static const int pipe = getenv("TS_PIX_PIPE") ? atoi(getenv("TS_PIX_PIPE")) : 5;
@@ -1650,16 +1707,17 @@ void pixel_destroy(ts_engine* e) {
 
 void pixelcnn_generate_act(ts_engine* e, const Act3& aud, const int64_t* label, const float* noise, int64_t* idx_out,
                            float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s, bool logits_all,
-                           const SampleCtl* ctl) {
+                           const SampleCtl* ctl, const int64_t* seeds) {
   if (!e->pix) fail(TS_ERR_NOT_LOADED, "pixelcnn weights not loaded");
-  generate_chunk(e, aud, 0, label, noise, B, idx_out, logits_out, B, T, pre, T0, s, logits_all, ctl);
+  generate_chunk(e, aud, 0, label, noise, B, idx_out, logits_out, B, T, pre, T0, s, logits_all, ctl, seeds);
 }
 
-void check_sample_ctl(const SampleCtl& c, const float* noise) {
+void check_sample_ctl(const SampleCtl& c, const float* noise, const int64_t* seeds) {
   if (!std::isfinite(c.temperature) || c.temperature < 0.f)
     fail(TS_ERR_INVALID, "pixelcnn sample: temperature %g (must be finite and >= 0)", (double)c.temperature);
   if (c.top_k < 0 || c.top_k > PIX_NCODE) fail(TS_ERR_INVALID, "pixelcnn sample: top_k %d outside [0, %d]", c.top_k, PIX_NCODE);
-  if (c.temperature > 0.f && !noise) fail(TS_ERR_INVALID, "pixelcnn sample: noise is NULL with temperature %g > 0", (double)c.temperature);
+  if (c.temperature > 0.f && !noise && !seeds)
+    fail(TS_ERR_INVALID, "pixelcnn sample: noise (or seeds) is NULL with temperature %g > 0", (double)c.temperature);
   if (!(c.top_p > 0.f && c.top_p <= 1.f)) fail(TS_ERR_INVALID, "pixelcnn sample: top_p %g outside (0, 1]", (double)c.top_p);
   if (!(c.min_p >= 0.f && c.min_p <= 1.f)) fail(TS_ERR_INVALID, "pixelcnn sample: min_p %g outside [0, 1]", (double)c.min_p);
 }
@@ -1799,18 +1857,19 @@ static void check_pix(ts_engine* e, int B, int T) {
   if (B <= 0 || T <= 0) fail(TS_ERR_INVALID, "pixelcnn: B=%d T=%d", B, T);
 }
 
-// ctl = nullptr: the default sampler (ts_pixelcnn_generate); else the sampling controls of ts_pixelcnn_sample
+// ctl = nullptr: the default sampler (ts_pixelcnn_generate); else the sampling controls of ts_pixelcnn_sample.
+// seeds (ts_pixelcnn_sample_seeded): the draws' noise comes from the per-clip seeds instead of `noise`.
 static void pixelcnn_generate_call(ts_engine* e, const float* aud, const int64_t* label, const float* noise, int64_t* idx_out,
                                    float* logits_out, int B, int T, const int64_t* pre_latents, int T0, void* stream,
-                                   const SampleCtl* ctl) {
+                                   const SampleCtl* ctl, const int64_t* seeds = nullptr) {
   check_pix(e, B, T);
   if (T0 < 0 || (T0 > 0 && !pre_latents)) fail(TS_ERR_INVALID, "pixelcnn: T0=%d without pre_latents", T0);
-  if (ctl) check_sample_ctl(*ctl, noise);
+  if (ctl) check_sample_ctl(*ctl, noise, seeds);
   cudaStream_t s = (cudaStream_t)stream;
   auto body = [&] {
     Act3 a = new_act(e, B, T0 + T, 256, 0, s);
     nct_to_act(e, aud, 256, a, s);
-    pixelcnn_generate_act(e, a, label, noise, idx_out, logits_out, B, T, pre_latents, T0, s, false, ctl);
+    pixelcnn_generate_act(e, a, label, noise, idx_out, logits_out, B, T, pre_latents, T0, s, false, ctl, seeds);
   };
   e->ws.begin_sizing(); body();
   size_t need = e->ws.need;
@@ -1839,6 +1898,43 @@ extern "C" int ts_pixelcnn_sample_ctl(ts_engine* e, const float* aud, const int6
   TS_API_BEGIN(e)
   const SampleCtl c = sample_ctl_of(ctl);
   pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, &c);
+  TS_API_END(e)
+}
+
+// The Exp(1) values of the seeded sampler in the layout of `noise`: block (2 (r - T0) + c) B + m holds draw (r, c) of
+// clip m.  One CTA of 256 threads per block, the thread <-> code mapping of the samplers.
+__global__ void __launch_bounds__(256) sampler_noise_kernel(const int64_t* __restrict__ seeds, float* __restrict__ out, int B, int T0) {
+  const int blk = blockIdx.x, m = blk % B, step = blk / B;
+  float q[8];
+  seeded_q(seeds[m], T0 + (step >> 1), step & 1, threadIdx.x, q);
+  float* dst = out + (size_t)blk * PIX_NCODE;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) dst[threadIdx.x + 256 * j] = q[j];
+}
+
+extern "C" int ts_sampler_noise(ts_engine* e, const int64_t* seeds, float* noise_out, int B, int T, int T0, void* stream) {
+  TS_API_BEGIN(e)
+  ts::require_device(e);
+  if (B <= 0 || T <= 0 || T0 < 0 || (int64_t)2 * T * B > INT32_MAX || !seeds || !noise_out)
+    fail(TS_ERR_INVALID, "ts_sampler_noise: B=%d T=%d T0=%d seeds=%p noise_out=%p", B, T, T0, (const void*)seeds, (void*)noise_out);
+  sampler_noise_kernel<<<2 * T * B, 256, 0, (cudaStream_t)stream>>>(seeds, noise_out, B, T0);
+  e->launches++;
+  TS_CUDA(cudaGetLastError());
+  TS_API_END(e)
+}
+
+extern "C" int ts_pixelcnn_sample_seeded(ts_engine* e, const float* aud, const int64_t* label, const int64_t* seeds,
+                                         int64_t* idx_out, float* logits_out, int B, int T, const int64_t* pre_latents, int T0,
+                                         const ts_sample_ctl* ctl, void* stream) {
+  TS_API_BEGIN(e)
+  check_pix(e, B, T);
+  if (ctl) {
+    const SampleCtl c = sample_ctl_of(ctl);
+    pixelcnn_generate_call(e, aud, label, nullptr, idx_out, logits_out, B, T, pre_latents, T0, stream, &c, seeds);
+  } else {
+    if (!seeds) fail(TS_ERR_INVALID, "ts_pixelcnn_sample_seeded: seeds is NULL (only greedy decoding runs without)");
+    pixelcnn_generate_call(e, aud, label, nullptr, idx_out, logits_out, B, T, pre_latents, T0, stream, nullptr, seeds);
+  }
   TS_API_END(e)
 }
 

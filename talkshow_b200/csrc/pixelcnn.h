@@ -82,15 +82,16 @@ struct SampleCtl {
   int* kept_out = nullptr;   // [B,T,2] size of each draw's final keep set, or null
 };
 // Validates the controls (TS_ERR_INVALID): temperature finite and >= 0, top_k in [0, 2048], top_p in (0, 1], min_p in
-// [0, 1], noise given when sampling.
-void check_sample_ctl(const SampleCtl& c, const float* noise);
+// [0, 1], noise (or seeds) given when sampling.
+void check_sample_ctl(const SampleCtl& c, const float* noise, const int64_t* seeds = nullptr);
 // The public struct as the internal one (TS_ERR_INVALID when null).
 SampleCtl sample_ctl_of(const ts_sample_ctl* c);
 
-// aud: AudioEncoder output, channel-last [B, T0+T, 256].  ctl = nullptr: the default sampler.
+// aud: AudioEncoder output, channel-last [B, T0+T, 256].  ctl = nullptr: the default sampler.  seeds [B] (device): the
+// draws' noise is computed from the per-clip seeds (ts_pixelcnn_sample_seeded) and `noise` is not read.
 void pixelcnn_generate_act(ts_engine* e, const Act3& aud, const int64_t* label, const float* noise, int64_t* idx_out,
                            float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s,
-                           bool logits_all = false, const SampleCtl* ctl = nullptr);
+                           bool logits_all = false, const SampleCtl* ctl = nullptr, const int64_t* seeds = nullptr);
 // idx [B,T,2] -> idx_c [2][B][T]; optionally copies idx to codes_out
 void split_codes(ts_engine* e, const int64_t* idx, int64_t* idx_c, int B, int T, int64_t* codes_out, cudaStream_t s);
 void pixel_destroy(ts_engine* e);

@@ -9,6 +9,7 @@ from __future__ import annotations
 import ctypes as C
 import math
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -53,12 +54,55 @@ def sample_controls(temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=
     return ctl
 
 
-def _controlled(temperature, top_k, noise, want_logp, top_p=1.0, min_p=0.0, want_kept=False):
-    """Engine side: validate the controls and the noise; True when the call leaves the default entry points."""
+def _wrap64(v):
+    """An integer as the int64 with the same low 64 bits."""
+    return (int(v) + (1 << 63)) % (1 << 64) - (1 << 63)
+
+
+def clip_seeds(seed, B):
+    """Per-clip seeds of a batch from one integer: ``seed + arange(B)`` wrapped to int64 bits, int64 [B] (host)."""
+    if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)):
+        raise ValueError("clip_seeds: seed must be an integer, got %r" % (seed,))
+    return torch.tensor([_wrap64(int(seed) + b) for b in range(int(B))], dtype=torch.int64)
+
+
+def check_seeds(seeds, B):
+    """Seeds of a seeded call as an int64 tensor [B]: an int64 tensor of shape [B] (host or device) is taken as it is, a
+    length-B sequence of integers is wrapped to int64 bits.  Any other shape, dtype or type raises ValueError."""
+    if torch.is_tensor(seeds):
+        if seeds.dtype != torch.int64 or tuple(seeds.shape) != (B,):
+            raise ValueError("seeds must be an int64 tensor of shape [%d], got %s %s" % (B, seeds.dtype, tuple(seeds.shape)))
+        return seeds
+    if isinstance(seeds, np.ndarray):
+        if seeds.dtype.kind not in "iu" or seeds.shape != (B,):
+            raise ValueError("seeds must be an integer array of shape [%d], got %s %s" % (B, seeds.dtype, seeds.shape))
+        seeds = seeds.tolist()
+    if isinstance(seeds, (str, bytes)) or not hasattr(seeds, "__len__") or len(seeds) != B:
+        raise ValueError("seeds must be a sequence of %d integers or an int64 tensor [%d], got %r" % (B, B, seeds))
+    if any(isinstance(s, bool) or not isinstance(s, (int, np.integer)) for s in seeds):
+        raise ValueError("seeds must be integers, got %r" % (seeds,))
+    return torch.tensor([_wrap64(s) for s in seeds], dtype=torch.int64)
+
+
+def resolve_clip_seeds(value, B):
+    """The ``clip_seeds=`` keyword of the wrappers: None stays None, an integer means ``clip_seeds(value, B)``, a length-B
+    sequence or tensor gives one seed per clip (``check_seeds``)."""
+    if value is None:
+        return None
+    if isinstance(value, (int, np.integer)) and not isinstance(value, bool):
+        return clip_seeds(value, B)
+    return check_seeds(value, B)
+
+
+def _controlled(temperature, top_k, noise, want_logp, top_p=1.0, min_p=0.0, want_kept=False, seeds=None):
+    """Engine side: validate the controls and the noise source; True when the call leaves the default entry points.
+    Sampling takes exactly one of ``noise`` and ``seeds``; greedy decoding needs neither."""
     check_sample_controls(temperature, top_k, top_p, min_p)
-    if noise is None and float(temperature) > 0:
-        raise ValueError("sampling at temperature %g needs the noise tensor (only greedy decoding, temperature 0, "
-                         "runs without)" % float(temperature))
+    if noise is not None and seeds is not None:
+        raise ValueError("give the sampler either noise or seeds, not both")
+    if noise is None and seeds is None and float(temperature) > 0:
+        raise ValueError("sampling at temperature %g needs the noise tensor or per-clip seeds (only greedy decoding, "
+                         "temperature 0, runs without)" % float(temperature))
     return bool(sample_controls(temperature, top_k, want_logp, top_p, min_p)) or bool(want_kept)
 
 
@@ -217,8 +261,24 @@ class Engine:
         self._check(self.L.ts_audio_encode(self.h, _lib.ptr(mfcc), _lib.ptr(out), B, M, self._s()), "ts_audio_encode")
         return out
 
+    def sampler_noise(self, seeds, T, T0=0):
+        """The Exp(1) values the seeded sampler uses (ts_sampler_noise): seeds [B] (``check_seeds``) -> [2T,B,2048] in the
+        layout of ``noise``, block 2(r-T0)+c for the rows r in [T0, T0+T)."""
+        if isinstance(T, bool) or int(T) != T or T < 1 or isinstance(T0, bool) or int(T0) != T0 or T0 < 0:
+            raise ValueError("sampler_noise: T=%r T0=%r (T >= 1, T0 >= 0)" % (T, T0))
+        try:
+            n = len(seeds)
+        except TypeError:
+            raise ValueError("sampler_noise: seeds must be a sequence of integers or an int64 tensor [B], got %r" % (seeds,))
+        seeds = self._dev(check_seeds(seeds, n), torch.int64)
+        B = seeds.shape[0]
+        out = torch.empty(2 * int(T), B, NCODE, device=self.device)
+        self._check(self.L.ts_sampler_noise(self.h, _lib.ptr(seeds), _lib.ptr(out), B, int(T), int(T0), self._s()),
+                    "ts_sampler_noise")
+        return out
+
     def pixelcnn_generate(self, aud, label, noise, T=None, pre_latents=None, want_logits=False, temperature=1.0, top_k=0,
-                          want_logp=False, top_p=1.0, min_p=0.0, want_kept=False):
+                          want_logp=False, top_p=1.0, min_p=0.0, want_kept=False, seeds=None):
         """GatedPixelCNN.generate: aud [B,256,T0+T], label [B], noise [2T,B,2048] -> codes [B,T,2]
         (+ logits [2T,B,2048]).  Batches above the 64-sample tile are chunked here.
 
@@ -229,12 +289,17 @@ class Engine:
 
         ``top_p`` (1 = off) and ``min_p`` (0 = off) truncate the draw further (nucleus / min-p sampling, in the order
         temperature, top_k, top_p, min_p; ts_pixelcnn_sample_ctl); ``want_kept`` appends kept [B,T,2] int32, the number
-        of codes each draw chose among."""
-        ctl = _controlled(temperature, top_k, noise, want_logp, top_p, min_p, want_kept)
+        of codes each draw chose among.
+
+        ``seeds`` [B] (``check_seeds``) replaces ``noise`` (pass None): seeded sampling, each clip's noise generated in the
+        sampler from its own seed and the absolute row of the draw (ts_pixelcnn_sample_seeded; RNG contract in
+        include/talkshow_b200.h).  Sampling takes exactly one of the two."""
+        ctl = _controlled(temperature, top_k, noise, want_logp, top_p, min_p, want_kept, seeds)
         aud = self._dev(aud, torch.float32)
         label = self._dev(label, torch.int64)
         noise = None if noise is None else self._dev(noise, torch.float32)
         B = aud.shape[0]
+        seeds = None if seeds is None else self._dev(check_seeds(seeds, B), torch.int64)
         T0 = 0 if pre_latents is None else pre_latents.shape[1]
         T = aud.shape[2] - T0 if T is None else T
         if label.numel() == 1 and B > 1:
@@ -257,7 +322,12 @@ class Engine:
             kz = kept if (full or kept is None) else torch.empty(nb, T, 2, dtype=torch.int32, device=self.device)
             args = (self.h, _lib.ptr(aud[b0:b1].contiguous()), _lib.ptr(label[b0:b1].contiguous()), _lib.ptr(nz),
                     _lib.ptr(cz), _lib.ptr(lz), nb, T, _lib.ptr(None if pre is None else pre[b0:b1].contiguous()), T0)
-            if ctl and _needs_ctl(top_p, min_p, want_kept):
+            if seeds is not None:
+                c = _ctl_struct(temperature, top_k, top_p, min_p, pz, kz) if ctl else None
+                args = args[:3] + (_lib.ptr(seeds[b0:b1]),) + args[4:]
+                self._check(self.L.ts_pixelcnn_sample_seeded(*args, None if c is None else C.byref(c), self._s()),
+                            "ts_pixelcnn_sample_seeded")
+            elif ctl and _needs_ctl(top_p, min_p, want_kept):
                 c = _ctl_struct(temperature, top_k, top_p, min_p, pz, kz)
                 self._check(self.L.ts_pixelcnn_sample_ctl(*args, C.byref(c), self._s()), "ts_pixelcnn_sample_ctl")
             elif ctl:
@@ -398,15 +468,17 @@ class Engine:
         return out
 
     def body_generate(self, mfcc, label, noise, want_codes=True, temperature=1.0, top_k=0, want_logp=False, top_p=1.0,
-                      min_p=0.0, want_kept=False):
+                      min_p=0.0, want_kept=False, seeds=None):
         """fused s2g_body_pixel core: mfcc [B,64,M] -> (codes [B,T,2], poses [B,4T,C]), C = 129 (258 for 6-D).
         Sampling controls as in ``pixelcnn_generate`` (ts_body_sample, ts_body_sample_ctl); ``want_logp`` appends logp
-        [B,T,2], ``want_kept`` then kept [B,T,2] int32."""
-        ctl = _controlled(temperature, top_k, noise, want_logp, top_p, min_p, want_kept)
+        [B,T,2], ``want_kept`` then kept [B,T,2] int32.  ``seeds`` [B] in place of ``noise``: seeded sampling
+        (ts_body_sample_seeded), as in ``pixelcnn_generate``."""
+        ctl = _controlled(temperature, top_k, noise, want_logp, top_p, min_p, want_kept, seeds)
         mfcc = self._dev(mfcc, torch.float32)
         label = self._dev(label, torch.int64)
         noise = None if noise is None else self._dev(noise, torch.float32)
         B, _, M = mfcc.shape
+        seeds = None if seeds is None else self._dev(check_seeds(seeds, B), torch.int64)
         if label.numel() == 1 and B > 1:
             label = label.expand(B).contiguous()
         T = self.latent_rows(M)
@@ -420,7 +492,15 @@ class Engine:
             nz = noise if (full or noise is None) else noise[:, b0:b1].contiguous()
             args = (self.h, _lib.ptr(mfcc[b0:b1]), _lib.ptr(label[b0:b1]), _lib.ptr(nz),
                     _lib.ptr(None if codes is None else codes[b0:b1]), _lib.ptr(poses[b0:b1]), b1 - b0, M)
-            if ctl and _needs_ctl(top_p, min_p, want_kept):
+            if seeds is not None:
+                c = None
+                if ctl:
+                    c = _ctl_struct(temperature, top_k, top_p, min_p, None if logp is None else logp[b0:b1],
+                                    None if kept is None else kept[b0:b1])
+                args = args[:3] + (_lib.ptr(seeds[b0:b1]),) + args[4:]
+                self._check(self.L.ts_body_sample_seeded(*args, None if c is None else C.byref(c), self._s()),
+                            "ts_body_sample_seeded")
+            elif ctl and _needs_ctl(top_p, min_p, want_kept):
                 c = _ctl_struct(temperature, top_k, top_p, min_p, None if logp is None else logp[b0:b1],
                                 None if kept is None else kept[b0:b1])
                 self._check(self.L.ts_body_sample_ctl(*args, C.byref(c), self._s()), "ts_body_sample_ctl")

@@ -10,7 +10,7 @@ import torch
 
 from ..data_utils.lower_body import c_index_3d, c_index_6d
 from ..data_utils.utils import get_mfcc_sepa, get_mfcc_ta, load_wav
-from ..engine import check_sample_controls, sample_controls
+from ..engine import check_sample_controls, resolve_clip_seeds, sample_controls
 from .base import draw_sampler_noise, resolve_device, shared_engine, strip_module
 
 
@@ -110,7 +110,9 @@ class TrainWrapper:
                        continuity=False, id=None, fps=15, sr=22000, B=1, am=None, am_sr=None, frame=0, **kwargs):
         """(aud_fn) -> generated motion, numpy (B, F, 129).  Reference: :232-289."""
         assert self.args.infer, "train mode"
-        ctl = {k: kwargs[k] for k in ("temperature", "top_k", "keep_logp", "top_p", "min_p") if k in kwargs}
+        ctl = {k: kwargs[k] for k in ("temperature", "top_k", "keep_logp", "top_p", "min_p", "clip_seeds") if k in kwargs}
+        if kwargs.get("noise_fn") is not None and kwargs.get("clip_seeds") is not None:
+            raise ValueError("infer_on_audio: noise_fn and clip_seeds are two noise sources; give one")
         if continuity:
             return self._infer_continuity(aud_fn, id, fps, sr, B, **ctl)
         if torch.is_tensor(aud_fn) or isinstance(aud_fn, np.ndarray):
@@ -125,7 +127,8 @@ class TrainWrapper:
         label = torch.tensor([0]) if id is None else id.reshape(-1).repeat(B)[:B] if id.numel() == 1 else id
         return self.generate(mfcc, label, noise_fn=kwargs.get("noise_fn"), **ctl).cpu().numpy()
 
-    def generate(self, aud, id, frame_num=0, noise_fn=None, temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0):
+    def generate(self, aud, id, frame_num=0, noise_fn=None, temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0,
+                 clip_seeds=None):
         """tensor API (:306-326): aud [B,64,M] features, id [B] -> torch (B, F, 129) on the device.
         (The reference's version passes decode()'s tuple to torch.cat and raises; this returns the
         tensor its infer_on_audio builds.)
@@ -134,38 +137,58 @@ class TrainWrapper:
         noise), ``top_k`` (0 = off); ``keep_logp`` keeps each draw's log-likelihood under the untempered prior as
         self.last_logp [B,T,2].  ``top_p`` (1 = off) and ``min_p`` (0 = off) add nucleus and min-p truncation; with
         ``keep_logp`` the number of codes each such draw chose among is kept as self.last_kept [B,T,2] (None when both are
-        off).  The defaults draw exactly like the reference."""
+        off).  The defaults draw exactly like the reference.
+
+        ``clip_seeds``: seeded sampling instead of torch-stream noise, so that a clip's motion depends only on its own seed
+        (not on B or its place in the batch).  An integer s seeds clip b with s + b (``engine.clip_seeds``); a length-B
+        sequence or int64 tensor gives each clip its seed.  Not combinable with ``noise_fn``."""
         mfcc = aud.to(torch.float32)
         B, _, M = mfcc.shape
         T = self.engine.latent_rows(M)
-        noise = self._draw_noise(T, B, noise_fn, temperature, top_k, top_p, min_p)
+        seeds = self._seeds(clip_seeds, B, noise_fn)
+        noise = self._draw_noise(T, B, noise_fn, temperature, top_k, top_p, min_p, seeds)
         ctl = sample_controls(temperature, top_k, keep_logp, top_p, min_p)
+        if noise is None and seeds is not None and float(temperature) > 0:
+            ctl["seeds"] = seeds
         out = self.engine.body_generate(mfcc, id.to(torch.int64), noise, **ctl)
         self.last_codes, poses = out[0], out[1]
         self.last_logp = out[2] if keep_logp else None
         self.last_kept = out[3] if ctl.get("want_kept") else None
         return poses
 
-    def _draw_noise(self, T, B, noise_fn, temperature, top_k, top_p=1.0, min_p=0.0):
-        """[2T,B,2048] Exp(1) draws (RNG contract), or None for greedy decoding (controls validated first)."""
+    def _draw_noise(self, T, B, noise_fn, temperature, top_k, top_p=1.0, min_p=0.0, seeds=None):
+        """[2T,B,2048] Exp(1) draws (RNG contract), or None for greedy decoding and seeded sampling (controls validated
+        first)."""
         check_sample_controls(temperature, top_k, top_p, min_p)
-        if float(temperature) == 0:
+        if float(temperature) == 0 or seeds is not None:
             return None
         return self._noise(T, B) if noise_fn is None else noise_fn(T, B)
 
+    @staticmethod
+    def _seeds(clip_seeds, B, noise_fn):
+        """``clip_seeds`` as int64 [B] (or None); ValueError with a noise_fn as well."""
+        if clip_seeds is not None and noise_fn is not None:
+            raise ValueError("noise_fn and clip_seeds are two noise sources; give one")
+        return resolve_clip_seeds(clip_seeds, B)
+
     def infer(self, aud_feat, frame, id, B, pre_latents=None, pre_audio=None, pre_pose=None, noise_fn=None,
-              temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0):
+              temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None):
         """The reference's inner call (:291-304): aud_feat [B,M,64] (time-major features of ONE chunk) ->
         (latents [B,T,2], audio [B,256,T,2], body [B,39,4T], hand [B,90,4T]).  ``pre_latents`` / ``pre_audio`` (the first
         two results of the previous chunk's call) condition the sampler on that chunk (GatedPixelCNN.generate :158-165);
         ``pre_pose`` is accepted and unused like in the reference, whose Decoder.forward ignores ``pre_state``
         (nets/spg/vqvae_1d.py:139-149) — each chunk is decoded on its own.  Sampling controls as in ``generate``; with
-        ``keep_logp`` the chunk's logp [B,T,2] is kept as self.last_logp (and its keep-set sizes as self.last_kept)."""
+        ``keep_logp`` the chunk's logp [B,T,2] is kept as self.last_logp (and its keep-set sizes as self.last_kept).
+        ``clip_seeds`` as in ``generate``; with ``pre_latents`` the chunk's draws are keyed by their absolute rows (after
+        the T0 rows of the previous chunk), so a seeded clip's noise does not depend on where it is cut into chunks."""
         a = self.engine.audio_encode(aud_feat.transpose(1, 2).contiguous())            # [B,256,T]
         T = a.shape[2]
         label = id.reshape(-1)
-        noise = self._draw_noise(T, B, noise_fn, temperature, top_k, top_p, min_p)
+        seeds = self._seeds(clip_seeds, B, noise_fn)
+        noise = self._draw_noise(T, B, noise_fn, temperature, top_k, top_p, min_p, seeds)
         ctl = sample_controls(temperature, top_k, keep_logp, top_p, min_p)
+        if noise is None and seeds is not None and float(temperature) > 0:
+            ctl["seeds"] = seeds
         if pre_latents is None:
             out = self.engine.pixelcnn_generate(a, label, noise, **ctl)
         else:

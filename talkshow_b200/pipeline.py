@@ -10,7 +10,7 @@ from __future__ import annotations
 
 import torch
 
-from .engine import Engine, sample_controls
+from .engine import Engine, resolve_clip_seeds, sample_controls
 from .nets.base import draw_sampler_noise
 
 
@@ -78,18 +78,25 @@ class WholeBody:
             self.e2 = None
 
     def generate(self, mfcc, wave, label, noise=None, stand=False, per_step_noise=True, temperature=1.0, top_k=0,
-                 keep_logp=False, top_p=1.0, min_p=0.0):
+                 keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None):
         """mfcc [B,64,M], wave [B,N] (16 kHz), label [B] on the device -> poses [B,F,265] (device).
         F = N*30//16000 face frames; the body (4*T frames) is padded/truncated to F like demo.py:207-211.
         Sampling controls of the body prior as in s2g_body_pixel.generate: ``temperature`` (0 = greedy, no noise is
         drawn), ``top_k``, ``top_p``, ``min_p``; ``keep_logp`` keeps each draw's log-likelihood under the untempered prior
-        as self.last_logp [B,T,2] and, with top_p or min_p on, the size of its keep set as self.last_kept [B,T,2]."""
+        as self.last_logp [B,T,2] and, with top_p or min_p on, the size of its keep set as self.last_kept [B,T,2].
+        ``clip_seeds`` (an integer s: clip b gets s + b; or a length-B sequence / int64 tensor): seeded sampling, no noise
+        is drawn and each clip's motion depends only on its seed.  Not combinable with ``noise``."""
         B, _, M = mfcc.shape
         frame = wave.shape[1] * 30 // 16000
         T = self.e.latent_rows(M)
         ctl = sample_controls(temperature, top_k, keep_logp, top_p, min_p)
         want_kept = bool(ctl.get("want_kept"))
-        if noise is None and float(temperature) > 0:
+        if noise is not None and clip_seeds is not None:
+            raise ValueError("WholeBody.generate: noise and clip_seeds are two noise sources; give one")
+        seeds = resolve_clip_seeds(clip_seeds, B)
+        if seeds is not None and float(temperature) > 0:
+            ctl["seeds"] = seeds
+        elif noise is None and float(temperature) > 0:
             noise = draw_sampler_noise(T, B, self.device, per_step=per_step_noise)
         idz = torch.zeros(B, 4, device=self.device)                    # demo.py:173-181: id not passed
         if self.e2 is not None and B <= self.overlap_batch:
@@ -109,7 +116,7 @@ class WholeBody:
                 self.last_logp.record_stream(cur)
             if want_kept:
                 self.last_kept.record_stream(cur)
-            for t in (mfcc, label, noise):
+            for t in (mfcc, label, noise, ctl.get("seeds")):
                 if torch.is_tensor(t) and t.is_cuda:
                     t.record_stream(self._side)                          # allocated here, consumed on the side stream
             return self.e.assemble_pose(face, body, stand)
@@ -154,14 +161,17 @@ class WholeBody:
         return None, dict(face_losses, **vq_losses, ce_loss=float(nll.double().mean()))
 
     def generate_sharded(self, mfcc, wave, label, rank, world, noise_full=None, seed=None, stand=False, gather=True,
-                         group=None, temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0):
+                         group=None, temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None):
         """Multi-GPU form of ``generate`` whose RESULT DOES NOT DEPEND ON ``world`` (SURVEY.md §8e): the arguments are
         the FULL batch (host or device tensors, identical on every rank), the sampler noise is drawn for the full batch in
         the reference's order — ``noise_full`` [2T,B,2048], or drawn here from ``seed`` on this rank's device generator
         (same seed on every rank gives every rank the same stream) — and rank r keeps the slice of its contiguous shard
         ``shard_range(B, r, world)``.  Each rank runs its shard; ONE all-gather rebuilds [B,F,265] everywhere.
         Sampling controls as in ``generate`` (greedy decoding draws no noise); with ``keep_logp`` self.last_logp holds
-        this rank's shard (and self.last_kept, as in ``generate``)."""
+        this rank's shard (and self.last_kept, as in ``generate``).
+        ``clip_seeds`` (as in ``generate``, for the full batch): seeded sampling; rank r passes the seeds of its shard and
+        draws no noise at all, and the gathered result equals ``generate`` with the same seeds on one GPU.  ``seed`` keeps
+        its meaning (the torch stream of the full-batch noise) and is not used with ``clip_seeds``."""
         B, _, M = mfcc.shape
         lo, hi = shard_range(B, rank, world)
         T = self.e.latent_rows(M)
@@ -170,7 +180,12 @@ class WholeBody:
         ctl = dict(temperature=temperature, top_k=top_k, keep_logp=keep_logp) if sc else {}
         if "top_p" in sc:
             ctl.update(top_p=top_p, min_p=min_p)
-        if noise_full is None and float(temperature) > 0:
+        if noise_full is not None and clip_seeds is not None:
+            raise ValueError("WholeBody.generate_sharded: noise_full and clip_seeds are two noise sources; give one")
+        seeds = resolve_clip_seeds(clip_seeds, B)
+        if seeds is not None:
+            ctl["clip_seeds"] = seeds[lo:hi]
+        elif noise_full is None and float(temperature) > 0:
             g = None
             if seed is not None:
                 g = torch.Generator(device=self.device)
