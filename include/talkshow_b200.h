@@ -160,6 +160,29 @@ int ts_sampler_noise(ts_engine* e, const int64_t* seeds, float* noise_out, int B
 int ts_pixelcnn_sample_seeded(ts_engine* e, const float* aud, const int64_t* label, const int64_t* seeds, int64_t* idx_out,
                               float* logits_out, int B, int T, const int64_t* pre_latents, int T0,
                               const ts_sample_ctl* ctl, void* stream);
+/* ---- anchored sampling: pin chosen draws to given codes, sample the rest --------------------------------------------
+ * anchors [B,T,2] int64 (device), laid out like idx_out over the sampled rows: with pre_latents, anchor row i is absolute
+ * row T0+i.  Per draw (clip, row, column):
+ *  - a value a in [0, 2048) PINS the draw: its code is a.  The code is written to idx_out, gathered into the embedding
+ *    like a drawn code and conditions every later draw.
+ *  - -1 samples the draw exactly as the call without anchors would (its noise or seeds, its controls).
+ *  - any other value is treated as -1 by the kernel, so malformed device data never reaches the embedding gather (the
+ *    Python layer rejects such values before the call).
+ *  - A pinned draw reads no noise.  noise keeps its [2T,B,2048] shape (a pinned draw's block is not used); seeded noise is
+ *    keyed by the absolute (row, column) as before.  Either way no sampled draw's noise changes.
+ *  - logp_out of a pinned draw: (l[a] - max l) - logf(sum exp(l - max l)) on its raw logits, the arithmetic and reduction
+ *    order of a sampled draw's logp (pinning a draw to the code it draws gives the same bits).  kept_out is 0 for a pinned
+ *    draw.  logits_out is written as usual.
+ *  - The prior is causal: a pinned code conditions the later draws only (later rows, and column 1 of its own row when it
+ *    is in column 0).  This is not bidirectional infilling: nothing before a pinned draw depends on it.
+ * An anchored call runs the kernels of ts_pixelcnn_sample_ctl (with ctl = NULL at temperature 1, top_k 0: the default
+ * draw's codes) with the launches of ts_pixelcnn_generate.  Exactly one of noise and seeds must be given unless ctl is
+ * greedy (temperature 0), even when every draw is pinned; otherwise TS_ERR_INVALID.  ctl may be NULL.  anchors = NULL:
+ * the call makes the launches of, and equals bit for bit, ts_pixelcnn_generate (noise, ctl NULL),
+ * ts_pixelcnn_sample_ctl (noise, ctl) or ts_pixelcnn_sample_seeded (seeds, ctl). */
+int ts_pixelcnn_sample_anchored(ts_engine* e, const float* aud, const int64_t* label, const float* noise, const int64_t* seeds,
+                                const int64_t* anchors, int64_t* idx_out, float* logits_out, int B, int T,
+                                const int64_t* pre_latents, int T0, const ts_sample_ctl* ctl, void* stream);
 /* GatedPixelCNN.forward (teacher forced), :130-150, for rows [0,T): logits_out [B,2048,T,2]. */
 int ts_pixelcnn_logits(ts_engine* e, const float* aud, const int64_t* label, const int64_t* codes,
                        float* logits_out, int B, int T, void* stream);
@@ -232,6 +255,12 @@ int ts_body_sample_ctl(ts_engine* e, const float* mfcc, const int64_t* label, co
  * decoding (TS_ERR_INVALID otherwise). */
 int ts_body_sample_seeded(ts_engine* e, const float* mfcc, const int64_t* label, const int64_t* seeds, int64_t* codes,
                           float* poses, int B, int M, const ts_sample_ctl* ctl, void* stream);
+/* ts_body_generate with the anchors of ts_pixelcnn_sample_anchored ([B,T,2], T = ts_latent_rows(M)); the poses are decoded
+ * from the resulting codes, pinned or drawn.  Same noise / seeds / ctl rules; anchors = NULL equals ts_body_generate,
+ * ts_body_sample_ctl or ts_body_sample_seeded. */
+int ts_body_sample_anchored(ts_engine* e, const float* mfcc, const int64_t* label, const float* noise, const int64_t* seeds,
+                            const int64_t* anchors, int64_t* codes, float* poses, int B, int M, const ts_sample_ctl* ctl,
+                            void* stream);
 
 /* Audio front-end of get_mfcc_ta, data_utils/utils.py:148-177 (SURVEY.md §8f-1): wave [B,N] mono at
  * `sr` Hz -> torchaudio Resample(sr, 22000) -> MFCC(64 coefficients, n_fft 2048, hop 734 = 30 fps, 256 HTK

@@ -473,6 +473,9 @@ struct PixArgs {
   int* kept_out;       // [B][Ttot-T0][2] or null
   // seeded sampling (ts_pixelcnn_sample_seeded): [B] per-clip seeds; the draw's q comes from seeded_q, noise is unread
   const int64_t* seeds;
+  // anchored sampling (ts_pixelcnn_sample_anchored), read by the WARP instantiations only: [B][Ttot-T0][2], a value in
+  // [0, 2048) pins the draw to that code, anything else samples it; or null
+  const int64_t* anchors;
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -1164,6 +1167,28 @@ __device__ __forceinline__ long long cta_first_argmax(const float (&l)[8], float
   return cta_argmax(bv, bi, sf, si, scode, bar);
 }
 
+// log p of code under the untempered, untruncated logits l with maximum mx: *logp_dst = (l[code] - mx) - logf(sum_raw),
+// sum_raw = sum exp(l - mx) summed in the default sampler's order (taken as given when have_sum).  Written by the thread
+// that owns the code.
+template <class Bar>
+__device__ __forceinline__ void draw_logp(const float (&l)[8], float mx, long long code, bool have_sum, float sum_raw, float* sf,
+                                          float* logp_dst, Bar bar) {
+  if (!have_sum) {
+    float s = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) s += expf(l[j] - mx);
+    sum_raw = cta_sum8(s, sf, bar);
+  }
+  if (threadIdx.x == (int)(code & 255)) {
+    // l[code >> 8] as a sum of selected terms: a plain select chain is turned into an indexed load of a local copy of l
+    const int jc = (int)(code >> 8);
+    float lc = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) lc += j == jc ? l[j] : 0.f;
+    *logp_dst = (lc - mx) - logf(sum_raw);
+  }
+}
+
 // One controlled draw over the raw logits l (include/talkshow_b200.h, ts_pixelcnn_sample):
 //   temperature 0: first-index argmax of l (q is not read);
 //   else s = l / temperature (IEEE division), codes below the k-th largest logit -> -inf, then the default draw
@@ -1254,23 +1279,32 @@ __device__ __forceinline__ long long draw_controlled(const float (&l)[8], const 
     n = cta_count8(n, si, bar);
     if (tid == 0) *kept_dst = greedy ? 1 : n;
   }
-  if (logp_dst) {
-    if (greedy || temperature != 1.f || truncate) {
-      float s = 0.f;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) s += expf(l[j] - mx);
-      sum_raw = cta_sum8(s, sf, bar);
-    }
-    if (tid == (int)(code & 255)) {
-      // l[code >> 8] as a sum of selected terms: a plain select chain is turned into an indexed load of a local copy of l
-      const int jc = (int)(code >> 8);
-      float lc = 0.f;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) lc += j == jc ? l[j] : 0.f;
-      *logp_dst = (lc - mx) - logf(sum_raw);
-    }
-  }
+  if (logp_dst) draw_logp(l, mx, code, !(greedy || temperature != 1.f || truncate), sum_raw, sf, logp_dst, bar);
   return code;
+}
+
+// A draw pinned to `code` (ts_pixelcnn_sample_anchored): no noise, no draw.  logp_dst gets the log p of draw_controlled's
+// tail on the same logits (the same max, sum and reduction order), kept_dst gets 0.  scratch: the first 16 words of red.
+template <class Bar>
+__device__ __forceinline__ void draw_pinned(const float (&l)[8], long long code, float* red, float* logp_dst, int* kept_dst,
+                                            Bar bar) {
+  if (kept_dst && threadIdx.x == 0) *kept_dst = 0;
+  if (logp_dst) {
+    float mx = l[0];
+#pragma unroll
+    for (int j = 1; j < 8; ++j) mx = fmaxf(mx, l[j]);
+    mx = cta_max8(mx, red, bar);
+    draw_logp(l, mx, code, false, 0.f, red, logp_dst, bar);
+  }
+}
+
+// The pin of draw `at` ([B][T][2] index) of an anchored call: the anchor when it lies in [0, 2048), else -1 (sampled).
+// Any other value samples, so malformed device data never reaches the embedding gather.
+template <class Args>
+__device__ __forceinline__ long long anchor_of(const Args& A, size_t at) {
+  if (!A.anchors) return -1;
+  const long long a = __ldg(A.anchors + at);
+  return (a >= 0 && a < PIX_NCODE) ? a : -1;
 }
 
 // ---- seeded noise: the RNG contract of ts_pixelcnn_sample_seeded (include/talkshow_b200.h) --------------------------
@@ -1347,18 +1381,24 @@ __device__ void run_sample_task(const PixTask& t, const PixArgs& A, int r, int m
   long long code;
   if constexpr (WARP) {
     if (!forced) {
-      float qv[8];
-      if (A.temperature > 0.f) {
-        if (QPRE) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) qv[j] = qpre[j];
-        } else {
-          draw_noise(A, r, c, m, qv);
-        }
-      }
       const size_t at = ((size_t)m * (A.Ttot - A.T0) + (r - A.T0)) * 2 + c;
-      code = draw_controlled(l, qv, A.temperature, A.top_k, A.top_p, A.min_p, red, A.logp_out ? A.logp_out + at : nullptr,
-                             A.kept_out ? A.kept_out + at : nullptr, CtaBar());
+      const long long pin = anchor_of(A, at);   // the same in every thread: a uniform branch
+      if (pin >= 0) {
+        code = pin;
+        draw_pinned(l, code, red, A.logp_out ? A.logp_out + at : nullptr, A.kept_out ? A.kept_out + at : nullptr, CtaBar());
+      } else {
+        float qv[8];
+        if (A.temperature > 0.f) {
+          if (QPRE) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) qv[j] = qpre[j];
+          } else {
+            draw_noise(A, r, c, m, qv);
+          }
+        }
+        code = draw_controlled(l, qv, A.temperature, A.top_k, A.top_p, A.min_p, red, A.logp_out ? A.logp_out + at : nullptr,
+                               A.kept_out ? A.kept_out + at : nullptr, CtaBar());
+      }
     } else {
       code = A.pre[((size_t)m * A.T0 + r) * 2 + c];
     }
@@ -1575,7 +1615,7 @@ __global__ void logits_to_ref_kernel(const float* __restrict__ in, float* __rest
 
 static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t* label, const float* noise, int noise_B,
                            int64_t* idx_out, float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s,
-                           bool logits_all, const SampleCtl* ctl, const int64_t* seeds) {
+                           bool logits_all, const SampleCtl* ctl, const int64_t* seeds, const int64_t* anchors) {
   PixelPlan* P = e->pix;
   Plan3* Q = (Plan3*)P->p3;
   const int Ttot = T0 + T, D = P->D;
@@ -1602,7 +1642,8 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
   (void)noise_B;
 
   if (v3) {   // cluster-resident executor (pixelcnn3.inc): any batch size, clusters of 16 CTAs per 4 / 8 samples
-    launch_pixelcnn3(e, P, Q, audv, audh, label, noise, idx_out, logits_out, B, T0, Ttot, pre, logits_all, arena3, MB3, s, ctl, seeds);
+    launch_pixelcnn3(e, P, Q, audv, audh, label, noise, idx_out, logits_out, B, T0, Ttot, pre, logits_all, arena3, MB3, s, ctl, seeds,
+                     anchors);
     return;
   }
   if (B > PIX_MB)
@@ -1634,6 +1675,7 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
   A.temperature = c.temperature; A.top_k = c.top_k; A.logp_out = c.logp_out;
   A.top_p = c.top_p; A.min_p = c.min_p; A.kept_out = c.kept_out;
   A.seeds = seeds;
+  A.anchors = anchors;
   if (e->pixel_mode == 0) {
     // A/B switch: 0 = burst loads + scalar FFMA, 4 = pipelined loads + scalar FFMA, 5 (default) = pipelined loads + paired FMAs (fma2)
     static const int pipe = getenv("TS_PIX_PIPE") ? atoi(getenv("TS_PIX_PIPE")) : 5;
@@ -1707,9 +1749,12 @@ void pixel_destroy(ts_engine* e) {
 
 void pixelcnn_generate_act(ts_engine* e, const Act3& aud, const int64_t* label, const float* noise, int64_t* idx_out,
                            float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s, bool logits_all,
-                           const SampleCtl* ctl, const int64_t* seeds) {
+                           const SampleCtl* ctl, const int64_t* seeds, const int64_t* anchors) {
   if (!e->pix) fail(TS_ERR_NOT_LOADED, "pixelcnn weights not loaded");
-  generate_chunk(e, aud, 0, label, noise, B, idx_out, logits_out, B, T, pre, T0, s, logits_all, ctl, seeds);
+  // an anchored call always runs the WARP kernels; without controls at temperature 1, top_k 0 (the default draw's bits)
+  const SampleCtl dflt;
+  if (anchors && !ctl) ctl = &dflt;
+  generate_chunk(e, aud, 0, label, noise, B, idx_out, logits_out, B, T, pre, T0, s, logits_all, ctl, seeds, anchors);
 }
 
 void check_sample_ctl(const SampleCtl& c, const float* noise, const int64_t* seeds) {
@@ -1720,6 +1765,13 @@ void check_sample_ctl(const SampleCtl& c, const float* noise, const int64_t* see
     fail(TS_ERR_INVALID, "pixelcnn sample: noise (or seeds) is NULL with temperature %g > 0", (double)c.temperature);
   if (!(c.top_p > 0.f && c.top_p <= 1.f)) fail(TS_ERR_INVALID, "pixelcnn sample: top_p %g outside (0, 1]", (double)c.top_p);
   if (!(c.min_p >= 0.f && c.min_p <= 1.f)) fail(TS_ERR_INVALID, "pixelcnn sample: min_p %g outside [0, 1]", (double)c.min_p);
+}
+
+void check_anchored_source(const SampleCtl* ctl, const float* noise, const int64_t* seeds, const char* who) {
+  const bool greedy = ctl && ctl->temperature == 0.f;
+  if (!greedy && (noise != nullptr) == (seeds != nullptr))
+    fail(TS_ERR_INVALID, "%s: noise=%p seeds=%p (give exactly one; only greedy decoding runs without)", who, (const void*)noise,
+         (const void*)seeds);
 }
 
 SampleCtl sample_ctl_of(const ts_sample_ctl* c) {
@@ -1861,7 +1913,7 @@ static void check_pix(ts_engine* e, int B, int T) {
 // seeds (ts_pixelcnn_sample_seeded): the draws' noise comes from the per-clip seeds instead of `noise`.
 static void pixelcnn_generate_call(ts_engine* e, const float* aud, const int64_t* label, const float* noise, int64_t* idx_out,
                                    float* logits_out, int B, int T, const int64_t* pre_latents, int T0, void* stream,
-                                   const SampleCtl* ctl, const int64_t* seeds = nullptr) {
+                                   const SampleCtl* ctl, const int64_t* seeds = nullptr, const int64_t* anchors = nullptr) {
   check_pix(e, B, T);
   if (T0 < 0 || (T0 > 0 && !pre_latents)) fail(TS_ERR_INVALID, "pixelcnn: T0=%d without pre_latents", T0);
   if (ctl) check_sample_ctl(*ctl, noise, seeds);
@@ -1869,7 +1921,7 @@ static void pixelcnn_generate_call(ts_engine* e, const float* aud, const int64_t
   auto body = [&] {
     Act3 a = new_act(e, B, T0 + T, 256, 0, s);
     nct_to_act(e, aud, 256, a, s);
-    pixelcnn_generate_act(e, a, label, noise, idx_out, logits_out, B, T, pre_latents, T0, s, false, ctl, seeds);
+    pixelcnn_generate_act(e, a, label, noise, idx_out, logits_out, B, T, pre_latents, T0, s, false, ctl, seeds, anchors);
   };
   e->ws.begin_sizing(); body();
   size_t need = e->ws.need;
@@ -1935,6 +1987,22 @@ extern "C" int ts_pixelcnn_sample_seeded(ts_engine* e, const float* aud, const i
     if (!seeds) fail(TS_ERR_INVALID, "ts_pixelcnn_sample_seeded: seeds is NULL (only greedy decoding runs without)");
     pixelcnn_generate_call(e, aud, label, nullptr, idx_out, logits_out, B, T, pre_latents, T0, stream, nullptr, seeds);
   }
+  TS_API_END(e)
+}
+
+// anchors [B,T,2] (device): draws pinned to a code in [0, 2048), the others sampled; NULL: the entry point of the same
+// noise, seeds and ctl (ts_pixelcnn_generate, _sample_ctl or _sample_seeded) with its launches and bits.
+extern "C" int ts_pixelcnn_sample_anchored(ts_engine* e, const float* aud, const int64_t* label, const float* noise,
+                                           const int64_t* seeds, const int64_t* anchors, int64_t* idx_out, float* logits_out,
+                                           int B, int T, const int64_t* pre_latents, int T0, const ts_sample_ctl* ctl,
+                                           void* stream) {
+  TS_API_BEGIN(e)
+  check_pix(e, B, T);
+  SampleCtl c;
+  if (ctl) c = sample_ctl_of(ctl);
+  check_anchored_source(ctl ? &c : nullptr, noise, seeds, "ts_pixelcnn_sample_anchored");
+  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, ctl ? &c : nullptr, seeds,
+                         anchors);
   TS_API_END(e)
 }
 

@@ -88,10 +88,15 @@ void check_sample_ctl(const SampleCtl& c, const float* noise, const int64_t* see
 SampleCtl sample_ctl_of(const ts_sample_ctl* c);
 
 // aud: AudioEncoder output, channel-last [B, T0+T, 256].  ctl = nullptr: the default sampler.  seeds [B] (device): the
-// draws' noise is computed from the per-clip seeds (ts_pixelcnn_sample_seeded) and `noise` is not read.
+// draws' noise is computed from the per-clip seeds (ts_pixelcnn_sample_seeded) and `noise` is not read.  anchors
+// [B,T,2] (device): the pinned draws of ts_pixelcnn_sample_anchored; the call then runs the WARP kernels, at the default
+// controls when ctl is null.
 void pixelcnn_generate_act(ts_engine* e, const Act3& aud, const int64_t* label, const float* noise, int64_t* idx_out,
                            float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s,
-                           bool logits_all = false, const SampleCtl* ctl = nullptr, const int64_t* seeds = nullptr);
+                           bool logits_all = false, const SampleCtl* ctl = nullptr, const int64_t* seeds = nullptr,
+                           const int64_t* anchors = nullptr);
+// The noise source of an anchored call (TS_ERR_INVALID): exactly one of noise and seeds unless ctl is greedy.
+void check_anchored_source(const SampleCtl* ctl, const float* noise, const int64_t* seeds, const char* who);
 // idx [B,T,2] -> idx_c [2][B][T]; optionally copies idx to codes_out
 void split_codes(ts_engine* e, const int64_t* idx, int64_t* idx_c, int B, int T, int64_t* codes_out, cudaStream_t s);
 void pixel_destroy(ts_engine* e);

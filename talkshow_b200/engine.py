@@ -94,6 +94,28 @@ def resolve_clip_seeds(value, B):
     return check_seeds(value, B)
 
 
+def check_anchors(anchors, B, T):
+    """Anchors of an anchored call as an int64 tensor [B,T,2] (host or device, as given): an int64 tensor or a numpy
+    integer array of that shape whose values lie in [-1, 2048) (-1 = sample the draw, a code = pin it).  Anything else
+    raises ValueError.  The value check of a device tensor reads one reduction back: one synchronisation."""
+    if isinstance(anchors, np.ndarray):
+        if anchors.dtype.kind not in "iu" or anchors.shape != (B, T, 2):
+            raise ValueError("anchors must be an integer array of shape [%d,%d,2], got %s %s" % (B, T, anchors.dtype, anchors.shape))
+        if anchors.size and (anchors.min() < -1 or anchors.max() >= NCODE):
+            raise ValueError("anchors must lie in [-1, %d) (-1 = sampled), got values in [%d, %d]"
+                             % (NCODE, anchors.min(), anchors.max()))
+        return torch.from_numpy(np.ascontiguousarray(anchors, dtype=np.int64))
+    if not torch.is_tensor(anchors):
+        raise ValueError("anchors must be an int64 tensor or an integer numpy array [%d,%d,2], got %r" % (B, T, type(anchors)))
+    if anchors.dtype != torch.int64 or tuple(anchors.shape) != (B, T, 2):
+        raise ValueError("anchors must be an int64 tensor of shape [%d,%d,2], got %s %s" % (B, T, anchors.dtype, tuple(anchors.shape)))
+    if anchors.numel():
+        lo, hi = (int(v) for v in torch.stack([anchors.min(), anchors.max()]).tolist())
+        if lo < -1 or hi >= NCODE:
+            raise ValueError("anchors must lie in [-1, %d) (-1 = sampled), got values in [%d, %d]" % (NCODE, lo, hi))
+    return anchors
+
+
 def _controlled(temperature, top_k, noise, want_logp, top_p=1.0, min_p=0.0, want_kept=False, seeds=None):
     """Engine side: validate the controls and the noise source; True when the call leaves the default entry points.
     Sampling takes exactly one of ``noise`` and ``seeds``; greedy decoding needs neither."""
@@ -278,7 +300,7 @@ class Engine:
         return out
 
     def pixelcnn_generate(self, aud, label, noise, T=None, pre_latents=None, want_logits=False, temperature=1.0, top_k=0,
-                          want_logp=False, top_p=1.0, min_p=0.0, want_kept=False, seeds=None):
+                          want_logp=False, top_p=1.0, min_p=0.0, want_kept=False, seeds=None, anchors=None):
         """GatedPixelCNN.generate: aud [B,256,T0+T], label [B], noise [2T,B,2048] -> codes [B,T,2]
         (+ logits [2T,B,2048]).  Batches above the 64-sample tile are chunked here.
 
@@ -293,7 +315,13 @@ class Engine:
 
         ``seeds`` [B] (``check_seeds``) replaces ``noise`` (pass None): seeded sampling, each clip's noise generated in the
         sampler from its own seed and the absolute row of the draw (ts_pixelcnn_sample_seeded; RNG contract in
-        include/talkshow_b200.h).  Sampling takes exactly one of the two."""
+        include/talkshow_b200.h).  Sampling takes exactly one of the two.
+
+        ``anchors`` [B,T,2] (``check_anchors``: int64 tensor, host or device, or integer numpy array) pins chosen draws:
+        a value in [0, 2048) is the code of that draw, -1 samples it as the call without anchors would, with the same
+        noise or seeds and controls (ts_pixelcnn_sample_anchored).  With ``pre_latents`` anchor row i is row T0+i.  A pinned
+        code conditions later draws only (the prior is causal).  Values are checked (ValueError); for a device tensor that
+        costs one synchronisation.  None forwards exactly what the call forwards without it."""
         ctl = _controlled(temperature, top_k, noise, want_logp, top_p, min_p, want_kept, seeds)
         aud = self._dev(aud, torch.float32)
         label = self._dev(label, torch.int64)
@@ -302,6 +330,7 @@ class Engine:
         seeds = None if seeds is None else self._dev(check_seeds(seeds, B), torch.int64)
         T0 = 0 if pre_latents is None else pre_latents.shape[1]
         T = aud.shape[2] - T0 if T is None else T
+        anchors = None if anchors is None else self._dev(check_anchors(anchors, B, T), torch.int64)
         if label.numel() == 1 and B > 1:
             label = label.expand(B).contiguous()
         pre = None if pre_latents is None else self._dev(pre_latents, torch.int64)
@@ -322,7 +351,12 @@ class Engine:
             kz = kept if (full or kept is None) else torch.empty(nb, T, 2, dtype=torch.int32, device=self.device)
             args = (self.h, _lib.ptr(aud[b0:b1].contiguous()), _lib.ptr(label[b0:b1].contiguous()), _lib.ptr(nz),
                     _lib.ptr(cz), _lib.ptr(lz), nb, T, _lib.ptr(None if pre is None else pre[b0:b1].contiguous()), T0)
-            if seeds is not None:
+            if anchors is not None:
+                c = _ctl_struct(temperature, top_k, top_p, min_p, pz, kz) if ctl else None
+                args = args[:3] + (_lib.ptr(nz), _lib.ptr(None if seeds is None else seeds[b0:b1]), _lib.ptr(anchors[b0:b1])) + args[4:]
+                self._check(self.L.ts_pixelcnn_sample_anchored(*args, None if c is None else C.byref(c), self._s()),
+                            "ts_pixelcnn_sample_anchored")
+            elif seeds is not None:
                 c = _ctl_struct(temperature, top_k, top_p, min_p, pz, kz) if ctl else None
                 args = args[:3] + (_lib.ptr(seeds[b0:b1]),) + args[4:]
                 self._check(self.L.ts_pixelcnn_sample_seeded(*args, None if c is None else C.byref(c), self._s()),
@@ -468,11 +502,12 @@ class Engine:
         return out
 
     def body_generate(self, mfcc, label, noise, want_codes=True, temperature=1.0, top_k=0, want_logp=False, top_p=1.0,
-                      min_p=0.0, want_kept=False, seeds=None):
+                      min_p=0.0, want_kept=False, seeds=None, anchors=None):
         """fused s2g_body_pixel core: mfcc [B,64,M] -> (codes [B,T,2], poses [B,4T,C]), C = 129 (258 for 6-D).
         Sampling controls as in ``pixelcnn_generate`` (ts_body_sample, ts_body_sample_ctl); ``want_logp`` appends logp
         [B,T,2], ``want_kept`` then kept [B,T,2] int32.  ``seeds`` [B] in place of ``noise``: seeded sampling
-        (ts_body_sample_seeded), as in ``pixelcnn_generate``."""
+        (ts_body_sample_seeded), as in ``pixelcnn_generate``.  ``anchors`` [B,T,2] pins draws as in ``pixelcnn_generate``
+        (ts_body_sample_anchored; one synchronisation for a device tensor); the poses decode the resulting codes."""
         ctl = _controlled(temperature, top_k, noise, want_logp, top_p, min_p, want_kept, seeds)
         mfcc = self._dev(mfcc, torch.float32)
         label = self._dev(label, torch.int64)
@@ -482,6 +517,7 @@ class Engine:
         if label.numel() == 1 and B > 1:
             label = label.expand(B).contiguous()
         T = self.latent_rows(M)
+        anchors = None if anchors is None else self._dev(check_anchors(anchors, B, T), torch.int64)
         codes = torch.empty(B, T, 2, dtype=torch.int64, device=self.device) if want_codes else None
         poses = torch.empty(B, 4 * T, self.vq_dim(0) + self.vq_dim(1), device=self.device)
         logp = torch.empty(B, T, 2, device=self.device) if want_logp else None
@@ -492,7 +528,16 @@ class Engine:
             nz = noise if (full or noise is None) else noise[:, b0:b1].contiguous()
             args = (self.h, _lib.ptr(mfcc[b0:b1]), _lib.ptr(label[b0:b1]), _lib.ptr(nz),
                     _lib.ptr(None if codes is None else codes[b0:b1]), _lib.ptr(poses[b0:b1]), b1 - b0, M)
-            if seeds is not None:
+            if anchors is not None:
+                c = None
+                if ctl:
+                    c = _ctl_struct(temperature, top_k, top_p, min_p, None if logp is None else logp[b0:b1],
+                                    None if kept is None else kept[b0:b1])
+                args = args[:3] + (_lib.ptr(nz), _lib.ptr(None if seeds is None else seeds[b0:b1]),
+                                   _lib.ptr(anchors[b0:b1])) + args[4:]
+                self._check(self.L.ts_body_sample_anchored(*args, None if c is None else C.byref(c), self._s()),
+                            "ts_body_sample_anchored")
+            elif seeds is not None:
                 c = None
                 if ctl:
                     c = _ctl_struct(temperature, top_k, top_p, min_p, None if logp is None else logp[b0:b1],

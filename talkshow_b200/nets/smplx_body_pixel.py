@@ -113,6 +113,11 @@ class TrainWrapper:
         ctl = {k: kwargs[k] for k in ("temperature", "top_k", "keep_logp", "top_p", "min_p", "clip_seeds") if k in kwargs}
         if kwargs.get("noise_fn") is not None and kwargs.get("clip_seeds") is not None:
             raise ValueError("infer_on_audio: noise_fn and clip_seeds are two noise sources; give one")
+        if kwargs.get("anchors") is not None:
+            if continuity:
+                raise ValueError("infer_on_audio: anchors are not supported with continuity=True (the clip is cut into "
+                                 "two chunks); anchor each chunk through infer()")
+            ctl["anchors"] = kwargs["anchors"]
         if continuity:
             return self._infer_continuity(aud_fn, id, fps, sr, B, **ctl)
         if torch.is_tensor(aud_fn) or isinstance(aud_fn, np.ndarray):
@@ -128,7 +133,7 @@ class TrainWrapper:
         return self.generate(mfcc, label, noise_fn=kwargs.get("noise_fn"), **ctl).cpu().numpy()
 
     def generate(self, aud, id, frame_num=0, noise_fn=None, temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0,
-                 clip_seeds=None):
+                 clip_seeds=None, anchors=None):
         """tensor API (:306-326): aud [B,64,M] features, id [B] -> torch (B, F, 129) on the device.
         (The reference's version passes decode()'s tuple to torch.cat and raises; this returns the
         tensor its infer_on_audio builds.)
@@ -141,7 +146,12 @@ class TrainWrapper:
 
         ``clip_seeds``: seeded sampling instead of torch-stream noise, so that a clip's motion depends only on its own seed
         (not on B or its place in the batch).  An integer s seeds clip b with s + b (``engine.clip_seeds``); a length-B
-        sequence or int64 tensor gives each clip its seed.  Not combinable with ``noise_fn``."""
+        sequence or int64 tensor gives each clip its seed.  Not combinable with ``noise_fn``.
+
+        ``anchors`` [B,T,2] (T latent rows; int64 tensor or integer numpy array): a code in [0, 2048) pins that draw,
+        -1 samples it (Engine.pixelcnn_generate).  The codes of the call, pinned and drawn, are kept as self.last_codes.
+        To keep part of a known motion: ``torch.stack(vq.encode(poses), -1)`` of an s2g_body_vq, with -1 where new motion
+        is wanted.  The prior is causal: a pinned code conditions the draws after it, not those before."""
         mfcc = aud.to(torch.float32)
         B, _, M = mfcc.shape
         T = self.engine.latent_rows(M)
@@ -150,6 +160,8 @@ class TrainWrapper:
         ctl = sample_controls(temperature, top_k, keep_logp, top_p, min_p)
         if noise is None and seeds is not None and float(temperature) > 0:
             ctl["seeds"] = seeds
+        if anchors is not None:
+            ctl["anchors"] = anchors
         out = self.engine.body_generate(mfcc, id.to(torch.int64), noise, **ctl)
         self.last_codes, poses = out[0], out[1]
         self.last_logp = out[2] if keep_logp else None
@@ -172,7 +184,7 @@ class TrainWrapper:
         return resolve_clip_seeds(clip_seeds, B)
 
     def infer(self, aud_feat, frame, id, B, pre_latents=None, pre_audio=None, pre_pose=None, noise_fn=None,
-              temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None):
+              temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None, anchors=None):
         """The reference's inner call (:291-304): aud_feat [B,M,64] (time-major features of ONE chunk) ->
         (latents [B,T,2], audio [B,256,T,2], body [B,39,4T], hand [B,90,4T]).  ``pre_latents`` / ``pre_audio`` (the first
         two results of the previous chunk's call) condition the sampler on that chunk (GatedPixelCNN.generate :158-165);
@@ -180,7 +192,9 @@ class TrainWrapper:
         (nets/spg/vqvae_1d.py:139-149) — each chunk is decoded on its own.  Sampling controls as in ``generate``; with
         ``keep_logp`` the chunk's logp [B,T,2] is kept as self.last_logp (and its keep-set sizes as self.last_kept).
         ``clip_seeds`` as in ``generate``; with ``pre_latents`` the chunk's draws are keyed by their absolute rows (after
-        the T0 rows of the previous chunk), so a seeded clip's noise does not depend on where it is cut into chunks."""
+        the T0 rows of the previous chunk), so a seeded clip's noise does not depend on where it is cut into chunks.
+        ``anchors`` [B,T,2] cover this chunk's T rows (as in ``generate``); with ``pre_latents`` they pin rows after the
+        prefix."""
         a = self.engine.audio_encode(aud_feat.transpose(1, 2).contiguous())            # [B,256,T]
         T = a.shape[2]
         label = id.reshape(-1)
@@ -189,6 +203,8 @@ class TrainWrapper:
         ctl = sample_controls(temperature, top_k, keep_logp, top_p, min_p)
         if noise is None and seeds is not None and float(temperature) > 0:
             ctl["seeds"] = seeds
+        if anchors is not None:
+            ctl["anchors"] = anchors
         if pre_latents is None:
             out = self.engine.pixelcnn_generate(a, label, noise, **ctl)
         else:

@@ -10,7 +10,7 @@ from __future__ import annotations
 
 import torch
 
-from .engine import Engine, resolve_clip_seeds, sample_controls
+from .engine import Engine, check_anchors, resolve_clip_seeds, sample_controls
 from .nets.base import draw_sampler_noise
 
 
@@ -78,14 +78,17 @@ class WholeBody:
             self.e2 = None
 
     def generate(self, mfcc, wave, label, noise=None, stand=False, per_step_noise=True, temperature=1.0, top_k=0,
-                 keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None):
+                 keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None, anchors=None, keep_codes=False):
         """mfcc [B,64,M], wave [B,N] (16 kHz), label [B] on the device -> poses [B,F,265] (device).
         F = N*30//16000 face frames; the body (4*T frames) is padded/truncated to F like demo.py:207-211.
         Sampling controls of the body prior as in s2g_body_pixel.generate: ``temperature`` (0 = greedy, no noise is
         drawn), ``top_k``, ``top_p``, ``min_p``; ``keep_logp`` keeps each draw's log-likelihood under the untempered prior
         as self.last_logp [B,T,2] and, with top_p or min_p on, the size of its keep set as self.last_kept [B,T,2].
         ``clip_seeds`` (an integer s: clip b gets s + b; or a length-B sequence / int64 tensor): seeded sampling, no noise
-        is drawn and each clip's motion depends only on its seed.  Not combinable with ``noise``."""
+        is drawn and each clip's motion depends only on its seed.  Not combinable with ``noise``.
+        ``anchors`` [B,T,2] pins draws of the body prior (s2g_body_pixel.generate: a code pins, -1 samples).
+        ``keep_codes`` keeps the body codes of the call, pinned and drawn, as self.last_codes [B,T,2] (None otherwise):
+        the codes a later call can anchor to."""
         B, _, M = mfcc.shape
         frame = wave.shape[1] * 30 // 16000
         T = self.e.latent_rows(M)
@@ -98,6 +101,8 @@ class WholeBody:
             ctl["seeds"] = seeds
         elif noise is None and float(temperature) > 0:
             noise = draw_sampler_noise(T, B, self.device, per_step=per_step_noise)
+        if anchors is not None:
+            ctl["anchors"] = anchors
         idz = torch.zeros(B, 4, device=self.device)                    # demo.py:173-181: id not passed
         if self.e2 is not None and B <= self.overlap_batch:
             # small batch: sampler (on overlap_ctas SMs, launched first) and face regressor (on the free TPCs) side by side
@@ -105,8 +110,9 @@ class WholeBody:
             self._side.wait_stream(cur)
             self._body_engine = self.e2
             with torch.cuda.stream(self._side):
-                out = self.e2.body_generate(mfcc, label, noise, want_codes=False, **ctl)
+                out = self.e2.body_generate(mfcc, label, noise, want_codes=keep_codes, **ctl)
             body = out[1]
+            self.last_codes = out[0]
             self.last_logp = out[2] if keep_logp else None
             self.last_kept = out[3] if want_kept else None
             face = self.e.face_forward(wave, idz, frame)
@@ -116,13 +122,16 @@ class WholeBody:
                 self.last_logp.record_stream(cur)
             if want_kept:
                 self.last_kept.record_stream(cur)
-            for t in (mfcc, label, noise, ctl.get("seeds")):
+            if keep_codes:
+                self.last_codes.record_stream(cur)
+            for t in (mfcc, label, noise, ctl.get("seeds"), ctl.get("anchors")):
                 if torch.is_tensor(t) and t.is_cuda:
                     t.record_stream(self._side)                          # allocated here, consumed on the side stream
             return self.e.assemble_pose(face, body, stand)
         self._body_engine = self.e
         face = self.e.face_forward(wave, idz, frame)
-        out = self.e.body_generate(mfcc, label, noise, want_codes=False, **ctl)
+        out = self.e.body_generate(mfcc, label, noise, want_codes=keep_codes, **ctl)
+        self.last_codes = out[0]
         self.last_logp = out[2] if keep_logp else None
         self.last_kept = out[3] if want_kept else None
         return self.e.assemble_pose(face, out[1], stand)
@@ -161,7 +170,8 @@ class WholeBody:
         return None, dict(face_losses, **vq_losses, ce_loss=float(nll.double().mean()))
 
     def generate_sharded(self, mfcc, wave, label, rank, world, noise_full=None, seed=None, stand=False, gather=True,
-                         group=None, temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None):
+                         group=None, temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None,
+                         anchors=None):
         """Multi-GPU form of ``generate`` whose RESULT DOES NOT DEPEND ON ``world`` (SURVEY.md §8e): the arguments are
         the FULL batch (host or device tensors, identical on every rank), the sampler noise is drawn for the full batch in
         the reference's order — ``noise_full`` [2T,B,2048], or drawn here from ``seed`` on this rank's device generator
@@ -171,7 +181,9 @@ class WholeBody:
         this rank's shard (and self.last_kept, as in ``generate``).
         ``clip_seeds`` (as in ``generate``, for the full batch): seeded sampling; rank r passes the seeds of its shard and
         draws no noise at all, and the gathered result equals ``generate`` with the same seeds on one GPU.  ``seed`` keeps
-        its meaning (the torch stream of the full-batch noise) and is not used with ``clip_seeds``."""
+        its meaning (the torch stream of the full-batch noise) and is not used with ``clip_seeds``.
+        ``anchors`` [B,T,2] (as in ``generate``, for the full batch): rank r passes the rows of its shard, so the gathered
+        result equals ``generate`` with the same anchors on one GPU."""
         B, _, M = mfcc.shape
         lo, hi = shard_range(B, rank, world)
         T = self.e.latent_rows(M)
@@ -183,6 +195,8 @@ class WholeBody:
         if noise_full is not None and clip_seeds is not None:
             raise ValueError("WholeBody.generate_sharded: noise_full and clip_seeds are two noise sources; give one")
         seeds = resolve_clip_seeds(clip_seeds, B)
+        if anchors is not None:
+            ctl["anchors"] = check_anchors(anchors, B, T)[lo:hi]
         if seeds is not None:
             ctl["clip_seeds"] = seeds[lo:hi]
         elif noise_full is None and float(temperature) > 0:
