@@ -183,6 +183,26 @@ int ts_pixelcnn_sample_seeded(ts_engine* e, const float* aud, const int64_t* lab
 int ts_pixelcnn_sample_anchored(ts_engine* e, const float* aud, const int64_t* label, const float* noise, const int64_t* seeds,
                                 const int64_t* anchors, int64_t* idx_out, float* logits_out, int B, int T,
                                 const int64_t* pre_latents, int T0, const ts_sample_ctl* ctl, void* stream);
+/* ---- styled sampling: per-row mixtures of the speaker embeddings ----------------------------------------------------
+ * style [B, Ttot, ncls] float32 (device), Ttot = T0 + T: every latent row the network sees, the pre_latents prefix
+ * included.  Row r of clip b holds the speaker weights w[b,r,0..ncls) of every position (row r, columns 0 and 1) of every
+ * layer.  At a gate of layer l, channel ch, position (b, r, .) the class term E_l[label[b]][ch] is replaced by
+ *     acc = w0 * E_l[0][ch];  acc = acc + w_s * E_l[s][ch]  for s = 1 .. ncls-1,
+ * every product and every sum rounded to fp32 with no FMA contraction (__fmul_rn / __fadd_rn).  A one-hot row gives
+ * exactly E_l[s][ch] (up to the sign of a zero), so a one-hot schedule of class s equals the call labelled s bit for bit.
+ *  - Weights are used as given: the kernel neither normalises nor checks them (every code stays in [0, 2048) whatever the
+ *    logits).  The Python layer rejects non-finite or negative weights, rows whose sum differs from 1 by more than 1e-5
+ *    and wrong shapes before any launch: only convex mixtures of the trained embeddings are offered.
+ *  - With style, label is not read and may be NULL.  ncls must equal the loaded prior's class count and be at most 16,
+ *    otherwise TS_ERR_INVALID (every shipped config has 4).  Without style, label is required.
+ *  - The prior stays causal: a draw at row r depends only on the style rows <= r.
+ * A styled call runs the kernels of an anchored call (noise, seeds, anchors and ctl keep their contracts) with its
+ * launches.  style = NULL: the call equals ts_pixelcnn_sample_anchored bit for bit, with the same launches, and ncls is
+ * not read. */
+int ts_pixelcnn_sample_styled(ts_engine* e, const float* aud, const int64_t* label, const float* style, int ncls,
+                              const float* noise, const int64_t* seeds, const int64_t* anchors, int64_t* idx_out,
+                              float* logits_out, int B, int T, const int64_t* pre_latents, int T0, const ts_sample_ctl* ctl,
+                              void* stream);
 /* GatedPixelCNN.forward (teacher forced), :130-150, for rows [0,T): logits_out [B,2048,T,2]. */
 int ts_pixelcnn_logits(ts_engine* e, const float* aud, const int64_t* label, const int64_t* codes,
                        float* logits_out, int B, int T, void* stream);
@@ -193,6 +213,10 @@ int ts_pixelcnn_logits(ts_engine* e, const float* aud, const int64_t* label, con
  * Dense layers run on the kernel ts_set_tensor_cores selects. */
 int ts_pixelcnn_score(ts_engine* e, const float* aud, const int64_t* label, const int64_t* codes,
                       float* nll_out, float* logits_out, int B, int T, void* stream);
+/* ts_pixelcnn_score under a style schedule [B,T,ncls] (the rule of ts_pixelcnn_sample_styled: the gates of row t blend row
+ * t's weights, label is not read).  style = NULL equals ts_pixelcnn_score. */
+int ts_pixelcnn_score_styled(ts_engine* e, const float* aud, const int64_t* label, const float* style, int ncls,
+                             const int64_t* codes, float* nll_out, float* logits_out, int B, int T, void* stream);
 
 /* VQVAE.decode(latents=...), nets/spg/vqvae_1d.py:201-208: idx [B,T] int64 -> out [B,C,4T]
  * (C = ts_vq_dim(which): 39 body / 90 hand, 78 / 180 for 6-D).  The indices are device data and are NOT range-checked (the
@@ -261,6 +285,11 @@ int ts_body_sample_seeded(ts_engine* e, const float* mfcc, const int64_t* label,
 int ts_body_sample_anchored(ts_engine* e, const float* mfcc, const int64_t* label, const float* noise, const int64_t* seeds,
                             const int64_t* anchors, int64_t* codes, float* poses, int B, int M, const ts_sample_ctl* ctl,
                             void* stream);
+/* ts_body_sample_anchored under a style schedule [B,T,ncls] (T = ts_latent_rows(M); the rule of
+ * ts_pixelcnn_sample_styled, label may be NULL).  style = NULL equals ts_body_sample_anchored. */
+int ts_body_sample_styled(ts_engine* e, const float* mfcc, const int64_t* label, const float* style, int ncls,
+                          const float* noise, const int64_t* seeds, const int64_t* anchors, int64_t* codes, float* poses,
+                          int B, int M, const ts_sample_ctl* ctl, void* stream);
 
 /* Audio front-end of get_mfcc_ta, data_utils/utils.py:148-177 (SURVEY.md §8f-1): wave [B,N] mono at
  * `sr` Hz -> torchaudio Resample(sr, 22000) -> MFCC(64 coefficients, n_fft 2048, hop 734 = 30 fps, 256 HTK

@@ -65,6 +65,14 @@ SYMBOLS = {
                                               C.POINTER(ts_sample_ctl), C.c_void_p]),
     "ts_body_sample_anchored": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                           C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(ts_sample_ctl), C.c_void_p]),
+    "ts_pixelcnn_sample_styled": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                            C.c_int, C.POINTER(ts_sample_ctl), C.c_void_p]),
+    "ts_body_sample_styled": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(ts_sample_ctl),
+                                        C.c_void_p]),
+    "ts_pixelcnn_score_styled": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
     "ts_pixelcnn_logits": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                      C.c_void_p]),
     "ts_pixelcnn_score": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,

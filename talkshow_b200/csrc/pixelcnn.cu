@@ -476,7 +476,18 @@ struct PixArgs {
   // anchored sampling (ts_pixelcnn_sample_anchored), read by the WARP instantiations only: [B][Ttot-T0][2], a value in
   // [0, 2048) pins the draw to that code, anything else samples it; or null
   const int64_t* anchors;
+  // styled sampling (ts_pixelcnn_sample_styled), read by the WARP instantiations only: [B][Ttot][ncls] speaker weights per
+  // row, blended from cls_w [L][ncls][2D] at every gate in place of the CLS arena (style_pair); or null
+  const float* style;
+  const float* cls_w;
+  int ncls;
 };
+
+// The speaker weights of row r of clip m (global index) under A.style, or null for a padding sample (m >= B).
+template <class Args>
+__device__ __forceinline__ const float* style_row(const Args& A, int m, int r) {
+  return m < A.B ? A.style + ((size_t)m * A.Ttot + r) * A.ncls : nullptr;
+}
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
@@ -874,7 +885,10 @@ __device__ __forceinline__ EpiPre prefetch_epilogue(const PixTask& t, const PixA
   return p;
 }
 
-template <int PIPE, int MB, bool S2 = false>
+// WARP: a styled call (A.style) blends each gate's class term from row r's speaker weights; every gate a stage computes
+// at latent row r belongs to a position of row r (the vertical stack of row r reads rows < r only, the horizontal pass and
+// the forced prefix rows run at their own row), so row r of the schedule is the row of every gate here.
+template <int PIPE, int MB, bool S2 = false, bool WARP = false>
 __device__ void run_matmul_task(const PixTask& t, const PixArgs& A, int r, const float* Wsm, float* red, const EpiPre& pre) {
   constexpr int SEG = PIX_D * MB;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -939,6 +953,9 @@ __device__ void run_matmul_task(const PixTask& t, const PixArgs& A, int r, const
         float as = (t.K > 0 ? red_sum<MB>(red, 2 * j + 1, m) : 0.f) + bias[2 * j + 1];
         const float* cls = arena + a.CLS + (t.layer * 2) * SEG;
         float ct = cls[ax<MB>(q, m)], cs = cls[ax<MB>(PIX_D + q, m)];
+        if constexpr (WARP) {
+          if (A.style) style_pair(A.cls_w + (size_t)t.layer * A.ncls * 2 * PIX_D, style_row(A, m, r), A.ncls, PIX_D, q, ct, cs);
+        }
         if (t.epi == EPI_HGATE || t.epi == EPI_HGATE2) {
           const float* v2h = arena + a.V2H + ((t.layer * 2 + t.col) * 2) * SEG;
           float vt = pre.valid ? pre.a : __ldcg(v2h + ax<MB>(q, m));
@@ -1462,6 +1479,16 @@ __device__ void run_sample_task(const PixTask& t, const PixArgs& A, int r, int m
     // fused plan: layer-0 gate of column 1 (its matmul input is embedding[code] only -> gathered from T0)
     const float2 tw = *reinterpret_cast<const float2*>(A.blob + t.wofs + (size_t)code * (2 * PIX_D) + 2 * tid);
     const float* v2h = A.arena + A.lay.V2H + ((0 * 2 + 1) * 2) * SEG;
+    if constexpr (WARP) {
+      if (A.style) {   // position (r, 1): row r of the schedule
+        float ct, cs;
+        style_pair(A.cls_w, style_row(A, m, r), A.ncls, PIX_D, tid, ct, cs);
+        const float zt = (__ldcg(v2h + ax<MB>(tid, m)) + tw.x) + ct;
+        const float zs = (__ldcg(v2h + ax<MB>(PIX_D + tid, m)) + tw.y) + cs;
+        A.arena[A.lay.G + ax<MB>(tid, m)] = tanhf(zt) * sigmoidf_(zs);
+        return;
+      }
+    }
     const float* cls = A.arena + A.lay.CLS;
     const float zt = (__ldcg(v2h + ax<MB>(tid, m)) + tw.x) + cls[ax<MB>(tid, m)];
     const float zs = (__ldcg(v2h + ax<MB>(PIX_D + tid, m)) + tw.y) + cls[ax<MB>(PIX_D + tid, m)];
@@ -1500,7 +1527,7 @@ __global__ void __launch_bounds__(PIX_THREADS, 1) pixelcnn_kernel(PixArgs A, int
     for (int i = tid; i < nf; i += PIX_THREADS) wbuf[i] = A.blob[t.wofs + i];
     __syncthreads();
     EpiPre pre; pre.a = pre.b = 0.f; pre.valid = false;
-    run_matmul_task<0, MB, S2>(t, A, r_single, wbuf, red, pre);
+    run_matmul_task<0, MB, S2, WARP>(t, A, r_single, wbuf, red, pre);
     return;
   }
 
@@ -1559,7 +1586,7 @@ __global__ void __launch_bounds__(PIX_THREADS, 1) pixelcnn_kernel(PixArgs A, int
       if (t.epi == EPI_SAMPLE) {
         if (cta < A.B) run_sample_task<MB, true, WARP>(t, A, r, cta, red, qpre);
       }
-      else run_matmul_task<PIPE, MB, S2>(t, A, r, wbuf + buf * PIX_WBUF, red, pre);
+      else run_matmul_task<PIPE, MB, S2, WARP>(t, A, r, wbuf + buf * PIX_WBUF, red, pre);
     }
     if constexpr (TRACE) { __syncthreads(); if (tr) tr[2] = globaltimer_ns(); }
     grid_arrive(A.barrier);
@@ -1572,12 +1599,12 @@ __global__ void __launch_bounds__(PIX_THREADS, 1) pixelcnn_kernel(PixArgs A, int
 
 __global__ void build_cls_kernel(const float* __restrict__ cls_w, const int64_t* __restrict__ label, float* arena, int cls_off,
                                  int L, int ncls, int B, int MB) {
-  // CLS[l][ch][m] = class_cond_embedding_l[label[m]][ch]
+  // CLS[l][ch][m] = class_cond_embedding_l[label[m]][ch]; zero without a label (a styled call, which does not read CLS)
   int n = L * 2 * PIX_D * MB;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     int m = i % MB, ch = (i / MB) % (2 * PIX_D), l = i / (2 * PIX_D * MB);
     float v = 0.f;
-    if (m < B) {
+    if (m < B && label) {
       long long lb = label[m];
       lb = lb < 0 ? 0 : (lb >= ncls ? ncls - 1 : lb);
       v = cls_w[((size_t)l * ncls + lb) * 2 * PIX_D + ch];
@@ -1615,7 +1642,8 @@ __global__ void logits_to_ref_kernel(const float* __restrict__ in, float* __rest
 
 static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t* label, const float* noise, int noise_B,
                            int64_t* idx_out, float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s,
-                           bool logits_all, const SampleCtl* ctl, const int64_t* seeds, const int64_t* anchors) {
+                           bool logits_all, const SampleCtl* ctl, const int64_t* seeds, const int64_t* anchors,
+                           const float* style) {
   PixelPlan* P = e->pix;
   Plan3* Q = (Plan3*)P->p3;
   const int Ttot = T0 + T, D = P->D;
@@ -1643,7 +1671,7 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
 
   if (v3) {   // cluster-resident executor (pixelcnn3.inc): any batch size, clusters of 16 CTAs per 4 / 8 samples
     launch_pixelcnn3(e, P, Q, audv, audh, label, noise, idx_out, logits_out, B, T0, Ttot, pre, logits_all, arena3, MB3, s, ctl, seeds,
-                     anchors);
+                     anchors, style);
     return;
   }
   if (B > PIX_MB)
@@ -1676,6 +1704,7 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
   A.top_p = c.top_p; A.min_p = c.min_p; A.kept_out = c.kept_out;
   A.seeds = seeds;
   A.anchors = anchors;
+  A.style = style; A.cls_w = P->d_cls; A.ncls = P->nclasses;
   if (e->pixel_mode == 0) {
     // A/B switch: 0 = burst loads + scalar FFMA, 4 = pipelined loads + scalar FFMA, 5 (default) = pipelined loads + paired FMAs (fma2)
     static const int pipe = getenv("TS_PIX_PIPE") ? atoi(getenv("TS_PIX_PIPE")) : 5;
@@ -1749,12 +1778,24 @@ void pixel_destroy(ts_engine* e) {
 
 void pixelcnn_generate_act(ts_engine* e, const Act3& aud, const int64_t* label, const float* noise, int64_t* idx_out,
                            float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s, bool logits_all,
-                           const SampleCtl* ctl, const int64_t* seeds, const int64_t* anchors) {
+                           const SampleCtl* ctl, const int64_t* seeds, const int64_t* anchors, const float* style) {
   if (!e->pix) fail(TS_ERR_NOT_LOADED, "pixelcnn weights not loaded");
-  // an anchored call always runs the WARP kernels; without controls at temperature 1, top_k 0 (the default draw's bits)
+  // an anchored or styled call always runs the WARP kernels; without controls at temperature 1, top_k 0 (the default
+  // draw's bits)
   const SampleCtl dflt;
-  if (anchors && !ctl) ctl = &dflt;
-  generate_chunk(e, aud, 0, label, noise, B, idx_out, logits_out, B, T, pre, T0, s, logits_all, ctl, seeds, anchors);
+  if ((anchors || style) && !ctl) ctl = &dflt;
+  generate_chunk(e, aud, 0, label, noise, B, idx_out, logits_out, B, T, pre, T0, s, logits_all, ctl, seeds, anchors, style);
+}
+
+void check_style(const ts_engine* e, const int64_t* label, const float* style, int ncls, const char* who) {
+  if (!style) {
+    if (!label) fail(TS_ERR_INVALID, "%s: label is NULL without a style schedule", who);
+    return;
+  }
+  if (ncls < 1 || ncls > PIX_MAXCLS)
+    fail(TS_ERR_INVALID, "%s: ncls = %d (styled calls take 1 to %d classes)", who, ncls, PIX_MAXCLS);
+  if (ncls != e->pix->nclasses)
+    fail(TS_ERR_INVALID, "%s: ncls = %d, the loaded prior has %d classes", who, ncls, e->pix->nclasses);
 }
 
 void check_sample_ctl(const SampleCtl& c, const float* noise, const int64_t* seeds) {
@@ -1913,7 +1954,8 @@ static void check_pix(ts_engine* e, int B, int T) {
 // seeds (ts_pixelcnn_sample_seeded): the draws' noise comes from the per-clip seeds instead of `noise`.
 static void pixelcnn_generate_call(ts_engine* e, const float* aud, const int64_t* label, const float* noise, int64_t* idx_out,
                                    float* logits_out, int B, int T, const int64_t* pre_latents, int T0, void* stream,
-                                   const SampleCtl* ctl, const int64_t* seeds = nullptr, const int64_t* anchors = nullptr) {
+                                   const SampleCtl* ctl, const int64_t* seeds = nullptr, const int64_t* anchors = nullptr,
+                                   const float* style = nullptr) {
   check_pix(e, B, T);
   if (T0 < 0 || (T0 > 0 && !pre_latents)) fail(TS_ERR_INVALID, "pixelcnn: T0=%d without pre_latents", T0);
   if (ctl) check_sample_ctl(*ctl, noise, seeds);
@@ -1921,7 +1963,7 @@ static void pixelcnn_generate_call(ts_engine* e, const float* aud, const int64_t
   auto body = [&] {
     Act3 a = new_act(e, B, T0 + T, 256, 0, s);
     nct_to_act(e, aud, 256, a, s);
-    pixelcnn_generate_act(e, a, label, noise, idx_out, logits_out, B, T, pre_latents, T0, s, false, ctl, seeds, anchors);
+    pixelcnn_generate_act(e, a, label, noise, idx_out, logits_out, B, T, pre_latents, T0, s, false, ctl, seeds, anchors, style);
   };
   e->ws.begin_sizing(); body();
   size_t need = e->ws.need;
@@ -2003,6 +2045,23 @@ extern "C" int ts_pixelcnn_sample_anchored(ts_engine* e, const float* aud, const
   check_anchored_source(ctl ? &c : nullptr, noise, seeds, "ts_pixelcnn_sample_anchored");
   pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, ctl ? &c : nullptr, seeds,
                          anchors);
+  TS_API_END(e)
+}
+
+// style [B, T0+T, ncls] (device): per-row speaker weights blended into every gate's class term, label unread (may be
+// NULL); NULL: ts_pixelcnn_sample_anchored with its launches and bits.
+extern "C" int ts_pixelcnn_sample_styled(ts_engine* e, const float* aud, const int64_t* label, const float* style, int ncls,
+                                         const float* noise, const int64_t* seeds, const int64_t* anchors, int64_t* idx_out,
+                                         float* logits_out, int B, int T, const int64_t* pre_latents, int T0,
+                                         const ts_sample_ctl* ctl, void* stream) {
+  TS_API_BEGIN(e)
+  check_pix(e, B, T);
+  check_style(e, label, style, ncls, "ts_pixelcnn_sample_styled");
+  SampleCtl c;
+  if (ctl) c = sample_ctl_of(ctl);
+  check_anchored_source(ctl ? &c : nullptr, noise, seeds, "ts_pixelcnn_sample_styled");
+  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, ctl ? &c : nullptr, seeds,
+                         anchors, style);
   TS_API_END(e)
 }
 

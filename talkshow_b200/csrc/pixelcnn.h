@@ -90,11 +90,34 @@ SampleCtl sample_ctl_of(const ts_sample_ctl* c);
 // aud: AudioEncoder output, channel-last [B, T0+T, 256].  ctl = nullptr: the default sampler.  seeds [B] (device): the
 // draws' noise is computed from the per-clip seeds (ts_pixelcnn_sample_seeded) and `noise` is not read.  anchors
 // [B,T,2] (device): the pinned draws of ts_pixelcnn_sample_anchored; the call then runs the WARP kernels, at the default
-// controls when ctl is null.
+// controls when ctl is null.  style [B,T0+T,ncls] (device): the speaker schedule of ts_pixelcnn_sample_styled (label
+// unread), likewise on the WARP kernels.
 void pixelcnn_generate_act(ts_engine* e, const Act3& aud, const int64_t* label, const float* noise, int64_t* idx_out,
                            float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s,
                            bool logits_all = false, const SampleCtl* ctl = nullptr, const int64_t* seeds = nullptr,
-                           const int64_t* anchors = nullptr);
+                           const int64_t* anchors = nullptr, const float* style = nullptr);
+// The class terms of gate channel q (tanh half) and D + q (sigmoid half) under one row's speaker weights w[0..ncls)
+// (ts_pixelcnn_sample_styled): acc = w0 E[0][ch], then acc + w_s E[s][ch] for s = 1 .. ncls-1, every product and sum
+// rounded to fp32 without contraction.  tab: one layer's class_cond_embedding [ncls][2D]; w null (a padding sample of the
+// tile): zero, as in the CLS arena.
+__device__ __forceinline__ void style_pair(const float* __restrict__ tab, const float* __restrict__ w, int ncls, int D, int q,
+                                           float& ct, float& cs) {
+  if (!w) { ct = 0.f; cs = 0.f; return; }
+  const float w0 = __ldg(w);
+  ct = __fmul_rn(w0, __ldg(tab + q));
+  cs = __fmul_rn(w0, __ldg(tab + D + q));
+  for (int s = 1; s < ncls; ++s) {
+    const float ws = __ldg(w + s);
+    const float* e = tab + (size_t)s * 2 * D;
+    ct = __fadd_rn(ct, __fmul_rn(ws, __ldg(e + q)));
+    cs = __fadd_rn(cs, __fmul_rn(ws, __ldg(e + D + q)));
+  }
+}
+// Styled calls blend at most this many classes (ts_pixelcnn_sample_styled).
+constexpr int PIX_MAXCLS = 16;
+// The class input of a styled entry point (TS_ERR_INVALID): without style a label is required; with style, ncls in
+// [1, PIX_MAXCLS] and equal to the loaded prior's class count.
+void check_style(const ts_engine* e, const int64_t* label, const float* style, int ncls, const char* who);
 // The noise source of an anchored call (TS_ERR_INVALID): exactly one of noise and seeds unless ctl is greedy.
 void check_anchored_source(const SampleCtl* ctl, const float* noise, const int64_t* seeds, const char* who);
 // idx [B,T,2] -> idx_c [2][B][T]; optionally copies idx to codes_out

@@ -175,17 +175,27 @@ __global__ void tf_embed_kernel(const int64_t* __restrict__ codes, const float* 
   }
 }
 
-// GatedActivation (:16-22) of x + class_cond_embedding[label]: y = tanh(x[:D] + h[:D]) * sigmoid(x[D:] + h[D:])
-__global__ void tf_gate_kernel(Act3 x, const float* __restrict__ cls, const int64_t* __restrict__ label, int ncls, Act3 y) {
+// GatedActivation (:16-22) of x + class_cond_embedding[label]: y = tanh(x[:D] + h[:D]) * sigmoid(x[D:] + h[D:]).
+// style [B][T][ncls] (ts_pixelcnn_score_styled): h of cell (t, j) is the blend of row t's speaker weights (style_pair, the
+// sampler's fp32 order) and label is not read; null: the label's row.
+__global__ void tf_gate_kernel(Act3 x, const float* __restrict__ cls, const int64_t* __restrict__ label, int ncls, Act3 y,
+                               const float* __restrict__ style) {
   const int D = y.C;
   const long n = (long)y.B * y.T * D;
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
     const int o = i % D;
     const long cell = i / D;
     const int b = (int)(cell / y.T), t = (int)(cell % y.T);
-    const long lab = min(max(label[b], (int64_t)0), (int64_t)ncls - 1);
-    const float* h = cls + lab * 2 * D;
-    const float a = tf_load(x, b, t, o) + h[o], g = tf_load(x, b, t, D + o) + h[D + o];
+    float ht, hs;
+    if (style) {
+      style_pair(cls, style + ((size_t)b * (y.T >> 1) + (t >> 1)) * ncls, ncls, D, o, ht, hs);
+    } else {
+      const long lab = min(max(label[b], (int64_t)0), (int64_t)ncls - 1);
+      const float* h = cls + lab * 2 * D;
+      ht = h[o];
+      hs = h[D + o];
+    }
+    const float a = tf_load(x, b, t, o) + ht, g = tf_load(x, b, t, D + o) + hs;
     tf_store(y, b, t, o, tanhf(a) * (1.f / (1.f + expf(-g))));
   }
 }
@@ -229,8 +239,8 @@ __global__ void __launch_bounds__(TF_NLL_WARPS * 32) tf_nll_kernel(Act3 lg, cons
 static int tf_blocks(ts_engine* e, long n) { return (int)std::min<long>((n + 255) / 256, (long)e->sm_count * 16); }
 
 // ---- forward ----------------------------------------------------------------------------------
-static void tf_forward(ts_engine* e, const TfPlan* P, const float* aud, const int64_t* label, const int64_t* codes,
-                       float* nll, float* logits_out, int B, int T, cudaStream_t s) {
+static void tf_forward(ts_engine* e, const TfPlan* P, const float* aud, const int64_t* label, const float* style,
+                       const int64_t* codes, float* nll, float* logits_out, int B, int T, cudaStream_t s) {
   const int D = P->D, R = 2 * T;
   const bool sp = e->use_tc;   // GEMM operands stored in the split format the tensor-core kernel reads
   auto cells = [&](int C, int pad, bool split) { return new_act(e, B, R, C, pad, s, split); };
@@ -259,7 +269,7 @@ static void tf_forward(ts_engine* e, const TfPlan* P, const float* aud, const in
   Act3 xv[2] = {cells(D, TF_PAD, sp), cells(D, TF_PAD, sp)}, xh[2] = {cells(D, TF_PAD, sp), cells(D, TF_PAD, sp)};
   auto gate = [&](const Act3& x, int l, const Act3& y) {
     if (!run) return;
-    tf_gate_kernel<<<tf_blocks(e, (long)B * R * D), 256, 0, s>>>(x, P->cls + (size_t)l * P->ncls * 2 * D, label, P->ncls, y);
+    tf_gate_kernel<<<tf_blocks(e, (long)B * R * D), 256, 0, s>>>(x, P->cls + (size_t)l * P->ncls * 2 * D, label, P->ncls, y, style);
     e->launches++;
     TS_CUDA(cudaGetLastError());
   };
@@ -298,6 +308,19 @@ static void tf_forward(ts_engine* e, const TfPlan* P, const float* aud, const in
 
 using namespace ts;
 
+static void score_call(ts_engine* e, const float* aud, const int64_t* label, const float* style, const int64_t* codes,
+                       float* nll_out, float* logits_out, int B, int T, void* stream) {
+  const TfPlan* P = (const TfPlan*)e->pix->tf;
+  if (!P) fail(TS_ERR_NOT_LOADED, "pixelcnn scoring weights not loaded");
+  cudaStream_t s = (cudaStream_t)stream;
+  e->ws.begin_sizing();
+  tf_forward(e, P, aud, label, style, codes, nll_out, logits_out, B, T, s);
+  const size_t need = e->ws.need;
+  e->ws.buf.ensure(need + 256);
+  e->ws.begin(need);
+  tf_forward(e, P, aud, label, style, codes, nll_out, logits_out, B, T, s);
+}
+
 extern "C" int ts_pixelcnn_score(ts_engine* e, const float* aud, const int64_t* label, const int64_t* codes, float* nll_out,
                                  float* logits_out, int B, int T, void* stream) {
   TS_API_BEGIN(e)
@@ -305,14 +328,19 @@ extern "C" int ts_pixelcnn_score(ts_engine* e, const float* aud, const int64_t* 
   ts::require_device(e);
   if (B <= 0 || T <= 0) fail(TS_ERR_INVALID, "pixelcnn_score: B=%d T=%d", B, T);
   if (!aud || !label || !codes || !nll_out) fail(TS_ERR_INVALID, "pixelcnn_score: aud, label, codes and nll_out are required");
-  const TfPlan* P = (const TfPlan*)e->pix->tf;
-  if (!P) fail(TS_ERR_NOT_LOADED, "pixelcnn scoring weights not loaded");
-  cudaStream_t s = (cudaStream_t)stream;
-  e->ws.begin_sizing();
-  tf_forward(e, P, aud, label, codes, nll_out, logits_out, B, T, s);
-  const size_t need = e->ws.need;
-  e->ws.buf.ensure(need + 256);
-  e->ws.begin(need);
-  tf_forward(e, P, aud, label, codes, nll_out, logits_out, B, T, s);
+  score_call(e, aud, label, nullptr, codes, nll_out, logits_out, B, T, stream);
+  TS_API_END(e)
+}
+
+// style [B,T,ncls] (device): per-row speaker weights in place of label (which may then be NULL); NULL: ts_pixelcnn_score.
+extern "C" int ts_pixelcnn_score_styled(ts_engine* e, const float* aud, const int64_t* label, const float* style, int ncls,
+                                        const int64_t* codes, float* nll_out, float* logits_out, int B, int T, void* stream) {
+  TS_API_BEGIN(e)
+  if (!e->pix) fail(TS_ERR_NOT_LOADED, "pixelcnn weights not loaded");
+  ts::require_device(e);
+  if (B <= 0 || T <= 0) fail(TS_ERR_INVALID, "pixelcnn_score_styled: B=%d T=%d", B, T);
+  check_style(e, label, style, ncls, "ts_pixelcnn_score_styled");
+  if (!aud || !codes || !nll_out) fail(TS_ERR_INVALID, "pixelcnn_score_styled: aud, codes and nll_out are required");
+  score_call(e, aud, label, style, codes, nll_out, logits_out, B, T, stream);
   TS_API_END(e)
 }

@@ -116,6 +116,41 @@ def check_anchors(anchors, B, T):
     return anchors
 
 
+def check_style(style, B, Ttot, ncls):
+    """Speaker schedule of a styled call as a float32 tensor [B,Ttot,ncls] (host or device, as given): a float tensor or
+    numpy array of shape [B,Ttot,ncls], or [B,ncls] (one mixture per clip, broadcast over the rows).  It is converted to
+    float32 first and the float32 values are checked: finite, >= 0, each row summing to 1 within 1e-5 (a convex mixture of
+    the prior's trained speaker embeddings).  Anything else raises ValueError.  A device tensor costs one
+    synchronisation."""
+    if isinstance(style, np.ndarray):
+        if style.dtype.kind != "f":
+            raise ValueError("style must be a floating-point array, got %s" % (style.dtype,))
+        style = torch.from_numpy(np.ascontiguousarray(style))
+    if not torch.is_tensor(style):
+        raise ValueError("style must be a float tensor or numpy array [%d,%d,%d] or [%d,%d], got %r"
+                         % (B, Ttot, ncls, B, ncls, type(style)))
+    if not style.is_floating_point():
+        raise ValueError("style must be a floating-point tensor, got %s" % (style.dtype,))
+    shape = tuple(style.shape)
+    if shape == (B, ncls):
+        style = style[:, None, :].expand(B, Ttot, ncls)
+    elif shape != (B, Ttot, ncls):
+        raise ValueError("style must have shape [%d,%d,%d] (clips, rows, classes) or [%d,%d], got %s"
+                         % (B, Ttot, ncls, B, ncls, shape))
+    style = style.to(torch.float32).contiguous()
+    if style.numel():
+        w = style.double()
+        bad_sum = (w.sum(-1) - 1.0).abs().max()
+        ok = torch.stack([torch.isfinite(w).all().double(), (w >= 0).all().double(), bad_sum]).tolist()
+        if not ok[0]:
+            raise ValueError("style weights must be finite")
+        if not ok[1]:
+            raise ValueError("style weights must be >= 0 (convex mixtures only)")
+        if not ok[2] <= 1e-5:
+            raise ValueError("every style row must sum to 1 within 1e-5, worst row is off by %g" % ok[2])
+    return style
+
+
 def _controlled(temperature, top_k, noise, want_logp, top_p=1.0, min_p=0.0, want_kept=False, seeds=None):
     """Engine side: validate the controls and the noise source; True when the call leaves the default entry points.
     Sampling takes exactly one of ``noise`` and ``seeds``; greedy decoding needs neither."""
@@ -235,6 +270,7 @@ class Engine:
         arr, keep = _lib.pack_tensors(sd)
         self._check(self.L.ts_load_pixelcnn(self.h, arr, len(sd)), "ts_load_pixelcnn")
         self.loaded.add("pixelcnn")
+        self.pixelcnn_ncls = int(sd["layers.0.class_cond_embedding.weight"].shape[0])   # speaker classes (style=)
 
     def load_audioenc(self, sd):
         arr, keep = _lib.pack_tensors(sd)
@@ -300,7 +336,7 @@ class Engine:
         return out
 
     def pixelcnn_generate(self, aud, label, noise, T=None, pre_latents=None, want_logits=False, temperature=1.0, top_k=0,
-                          want_logp=False, top_p=1.0, min_p=0.0, want_kept=False, seeds=None, anchors=None):
+                          want_logp=False, top_p=1.0, min_p=0.0, want_kept=False, seeds=None, anchors=None, style=None):
         """GatedPixelCNN.generate: aud [B,256,T0+T], label [B], noise [2T,B,2048] -> codes [B,T,2]
         (+ logits [2T,B,2048]).  Batches above the 64-sample tile are chunked here.
 
@@ -321,17 +357,25 @@ class Engine:
         a value in [0, 2048) is the code of that draw, -1 samples it as the call without anchors would, with the same
         noise or seeds and controls (ts_pixelcnn_sample_anchored).  With ``pre_latents`` anchor row i is row T0+i.  A pinned
         code conditions later draws only (the prior is causal).  Values are checked (ValueError); for a device tensor that
-        costs one synchronisation.  None forwards exactly what the call forwards without it."""
+        costs one synchronisation.  None forwards exactly what the call forwards without it.
+
+        ``style`` (``check_style``: [B,T0+T,ncls] or [B,ncls], float) replaces the speaker label with a per-row convex
+        mixture of the prior's speaker embeddings (ts_pixelcnn_sample_styled; rule in include/talkshow_b200.h).  Its rows
+        cover every row the network sees, the ``pre_latents`` prefix included; ``label`` is then not read and may be None.
+        A one-hot schedule of class s draws what label s draws.  None forwards exactly what the call forwards without it."""
         ctl = _controlled(temperature, top_k, noise, want_logp, top_p, min_p, want_kept, seeds)
         aud = self._dev(aud, torch.float32)
-        label = self._dev(label, torch.int64)
-        noise = None if noise is None else self._dev(noise, torch.float32)
         B = aud.shape[0]
+        if label is None and style is None:
+            raise ValueError("pixelcnn_generate: label is required without style")
+        label = None if label is None else self._dev(label, torch.int64)
+        noise = None if noise is None else self._dev(noise, torch.float32)
         seeds = None if seeds is None else self._dev(check_seeds(seeds, B), torch.int64)
         T0 = 0 if pre_latents is None else pre_latents.shape[1]
         T = aud.shape[2] - T0 if T is None else T
         anchors = None if anchors is None else self._dev(check_anchors(anchors, B, T), torch.int64)
-        if label.numel() == 1 and B > 1:
+        style = None if style is None else self._dev(check_style(style, B, T0 + T, self.pixelcnn_ncls), torch.float32)
+        if label is not None and label.numel() == 1 and B > 1:
             label = label.expand(B).contiguous()
         pre = None if pre_latents is None else self._dev(pre_latents, torch.int64)
         codes = torch.empty(B, T, 2, dtype=torch.int64, device=self.device)
@@ -349,9 +393,16 @@ class Engine:
             lz = logits if (full or logits is None) else torch.empty(2 * T, nb, 2048, device=self.device)
             pz = logp if (full or logp is None) else torch.empty(nb, T, 2, device=self.device)
             kz = kept if (full or kept is None) else torch.empty(nb, T, 2, dtype=torch.int32, device=self.device)
-            args = (self.h, _lib.ptr(aud[b0:b1].contiguous()), _lib.ptr(label[b0:b1].contiguous()), _lib.ptr(nz),
+            args = (self.h, _lib.ptr(aud[b0:b1].contiguous()), _lib.ptr(None if label is None else label[b0:b1].contiguous()), _lib.ptr(nz),
                     _lib.ptr(cz), _lib.ptr(lz), nb, T, _lib.ptr(None if pre is None else pre[b0:b1].contiguous()), T0)
-            if anchors is not None:
+            if style is not None:
+                c = _ctl_struct(temperature, top_k, top_p, min_p, pz, kz) if ctl else None
+                args = args[:3] + (_lib.ptr(style[b0:b1]), self.pixelcnn_ncls, _lib.ptr(nz),
+                                   _lib.ptr(None if seeds is None else seeds[b0:b1]),
+                                   _lib.ptr(None if anchors is None else anchors[b0:b1])) + args[4:]
+                self._check(self.L.ts_pixelcnn_sample_styled(*args, None if c is None else C.byref(c), self._s()),
+                            "ts_pixelcnn_sample_styled")
+            elif anchors is not None:
                 c = _ctl_struct(temperature, top_k, top_p, min_p, pz, kz) if ctl else None
                 args = args[:3] + (_lib.ptr(nz), _lib.ptr(None if seeds is None else seeds[b0:b1]), _lib.ptr(anchors[b0:b1])) + args[4:]
                 self._check(self.L.ts_pixelcnn_sample_anchored(*args, None if c is None else C.byref(c), self._s()),
@@ -392,20 +443,30 @@ class Engine:
                                               B, T, self._s()), "ts_pixelcnn_logits")
         return out
 
-    def pixelcnn_score(self, aud, label, codes, want_logits=False):
+    def pixelcnn_score(self, aud, label, codes, want_logits=False, style=None):
         """Teacher-forced GatedPixelCNN.forward over all rows at once + per-position cross-entropy: aud [B,256,T],
-        label [B], codes [B,T,2] -> nll [B,T,2] = -log softmax(logits)[code] (+ logits [B,2048,T,2]).  Any batch size."""
+        label [B], codes [B,T,2] -> nll [B,T,2] = -log softmax(logits)[code] (+ logits [B,2048,T,2]).  Any batch size.
+        ``style`` ([B,T,ncls] or [B,ncls], ``check_style``): score under a speaker schedule (ts_pixelcnn_score_styled);
+        ``label`` is then not read and may be None."""
         aud = self._dev(aud, torch.float32)
-        label = self._dev(label, torch.int64).reshape(-1)
+        if label is None and style is None:
+            raise ValueError("pixelcnn_score: label is required without style")
+        label = None if label is None else self._dev(label, torch.int64).reshape(-1)
         codes = self._dev(codes, torch.int64)
         B, _, T = aud.shape
-        if label.numel() == 1 and B > 1:
+        if label is not None and label.numel() == 1 and B > 1:
             label = label.expand(B).contiguous()
-        if aud.shape[1] != 256 or tuple(codes.shape) != (B, T, 2) or label.numel() != B:
+        if aud.shape[1] != 256 or tuple(codes.shape) != (B, T, 2) or (label is not None and label.numel() != B):
             raise ValueError("pixelcnn_score: aud %s, label %s, codes %s (expected [B,256,T], [B], [B,T,2])"
                              % (tuple(aud.shape), tuple(label.shape), tuple(codes.shape)))
         nll = torch.empty(B, T, 2, device=self.device)
         logits = torch.empty(B, 2048, T, 2, device=self.device) if want_logits else None
+        if style is not None:
+            style = self._dev(check_style(style, B, T, self.pixelcnn_ncls), torch.float32)
+            self._check(self.L.ts_pixelcnn_score_styled(self.h, _lib.ptr(aud), _lib.ptr(label), _lib.ptr(style),
+                                                        self.pixelcnn_ncls, _lib.ptr(codes), _lib.ptr(nll), _lib.ptr(logits),
+                                                        B, T, self._s()), "ts_pixelcnn_score_styled")
+            return (nll, logits) if want_logits else nll
         self._check(self.L.ts_pixelcnn_score(self.h, _lib.ptr(aud), _lib.ptr(label), _lib.ptr(codes), _lib.ptr(nll),
                                              _lib.ptr(logits), B, T, self._s()), "ts_pixelcnn_score")
         return (nll, logits) if want_logits else nll
@@ -502,22 +563,27 @@ class Engine:
         return out
 
     def body_generate(self, mfcc, label, noise, want_codes=True, temperature=1.0, top_k=0, want_logp=False, top_p=1.0,
-                      min_p=0.0, want_kept=False, seeds=None, anchors=None):
+                      min_p=0.0, want_kept=False, seeds=None, anchors=None, style=None):
         """fused s2g_body_pixel core: mfcc [B,64,M] -> (codes [B,T,2], poses [B,4T,C]), C = 129 (258 for 6-D).
         Sampling controls as in ``pixelcnn_generate`` (ts_body_sample, ts_body_sample_ctl); ``want_logp`` appends logp
         [B,T,2], ``want_kept`` then kept [B,T,2] int32.  ``seeds`` [B] in place of ``noise``: seeded sampling
         (ts_body_sample_seeded), as in ``pixelcnn_generate``.  ``anchors`` [B,T,2] pins draws as in ``pixelcnn_generate``
-        (ts_body_sample_anchored; one synchronisation for a device tensor); the poses decode the resulting codes."""
+        (ts_body_sample_anchored; one synchronisation for a device tensor); the poses decode the resulting codes.
+        ``style`` [B,T,ncls] or [B,ncls]: a speaker schedule as in ``pixelcnn_generate`` (ts_body_sample_styled; label
+        may then be None)."""
         ctl = _controlled(temperature, top_k, noise, want_logp, top_p, min_p, want_kept, seeds)
         mfcc = self._dev(mfcc, torch.float32)
-        label = self._dev(label, torch.int64)
+        if label is None and style is None:
+            raise ValueError("body_generate: label is required without style")
+        label = None if label is None else self._dev(label, torch.int64)
         noise = None if noise is None else self._dev(noise, torch.float32)
         B, _, M = mfcc.shape
         seeds = None if seeds is None else self._dev(check_seeds(seeds, B), torch.int64)
-        if label.numel() == 1 and B > 1:
+        if label is not None and label.numel() == 1 and B > 1:
             label = label.expand(B).contiguous()
         T = self.latent_rows(M)
         anchors = None if anchors is None else self._dev(check_anchors(anchors, B, T), torch.int64)
+        style = None if style is None else self._dev(check_style(style, B, T, self.pixelcnn_ncls), torch.float32)
         codes = torch.empty(B, T, 2, dtype=torch.int64, device=self.device) if want_codes else None
         poses = torch.empty(B, 4 * T, self.vq_dim(0) + self.vq_dim(1), device=self.device)
         logp = torch.empty(B, T, 2, device=self.device) if want_logp else None
@@ -526,9 +592,19 @@ class Engine:
             b1 = min(B, b0 + PIX_TILE)
             full = (b1 - b0) == B
             nz = noise if (full or noise is None) else noise[:, b0:b1].contiguous()
-            args = (self.h, _lib.ptr(mfcc[b0:b1]), _lib.ptr(label[b0:b1]), _lib.ptr(nz),
+            args = (self.h, _lib.ptr(mfcc[b0:b1]), _lib.ptr(None if label is None else label[b0:b1]), _lib.ptr(nz),
                     _lib.ptr(None if codes is None else codes[b0:b1]), _lib.ptr(poses[b0:b1]), b1 - b0, M)
-            if anchors is not None:
+            if style is not None:
+                c = None
+                if ctl:
+                    c = _ctl_struct(temperature, top_k, top_p, min_p, None if logp is None else logp[b0:b1],
+                                    None if kept is None else kept[b0:b1])
+                args = args[:3] + (_lib.ptr(style[b0:b1]), self.pixelcnn_ncls, _lib.ptr(nz),
+                                   _lib.ptr(None if seeds is None else seeds[b0:b1]),
+                                   _lib.ptr(None if anchors is None else anchors[b0:b1])) + args[4:]
+                self._check(self.L.ts_body_sample_styled(*args, None if c is None else C.byref(c), self._s()),
+                            "ts_body_sample_styled")
+            elif anchors is not None:
                 c = None
                 if ctl:
                     c = _ctl_struct(temperature, top_k, top_p, min_p, None if logp is None else logp[b0:b1],

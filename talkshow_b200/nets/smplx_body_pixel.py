@@ -10,7 +10,7 @@ import torch
 
 from ..data_utils.lower_body import c_index_3d, c_index_6d
 from ..data_utils.utils import get_mfcc_sepa, get_mfcc_ta, load_wav
-from ..engine import check_sample_controls, resolve_clip_seeds, sample_controls
+from ..engine import check_sample_controls, check_style, resolve_clip_seeds, sample_controls
 from .base import draw_sampler_noise, resolve_device, shared_engine, strip_module
 
 
@@ -118,6 +118,8 @@ class TrainWrapper:
                 raise ValueError("infer_on_audio: anchors are not supported with continuity=True (the clip is cut into "
                                  "two chunks); anchor each chunk through infer()")
             ctl["anchors"] = kwargs["anchors"]
+        if kwargs.get("style") is not None:
+            ctl["style"] = kwargs["style"]
         if continuity:
             return self._infer_continuity(aud_fn, id, fps, sr, B, **ctl)
         if torch.is_tensor(aud_fn) or isinstance(aud_fn, np.ndarray):
@@ -133,7 +135,7 @@ class TrainWrapper:
         return self.generate(mfcc, label, noise_fn=kwargs.get("noise_fn"), **ctl).cpu().numpy()
 
     def generate(self, aud, id, frame_num=0, noise_fn=None, temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0,
-                 clip_seeds=None, anchors=None):
+                 clip_seeds=None, anchors=None, style=None):
         """tensor API (:306-326): aud [B,64,M] features, id [B] -> torch (B, F, 129) on the device.
         (The reference's version passes decode()'s tuple to torch.cat and raises; this returns the
         tensor its infer_on_audio builds.)
@@ -151,7 +153,11 @@ class TrainWrapper:
         ``anchors`` [B,T,2] (T latent rows; int64 tensor or integer numpy array): a code in [0, 2048) pins that draw,
         -1 samples it (Engine.pixelcnn_generate).  The codes of the call, pinned and drawn, are kept as self.last_codes.
         To keep part of a known motion: ``torch.stack(vq.encode(poses), -1)`` of an s2g_body_vq, with -1 where new motion
-        is wanted.  The prior is causal: a pinned code conditions the draws after it, not those before."""
+        is wanted.  The prior is causal: a pinned code conditions the draws after it, not those before.
+
+        ``style`` [B,T,4] per-row or [B,4] per-clip speaker weights (Engine.check_style: convex mixtures, float): the
+        prior is conditioned on that mixture of its speaker embeddings instead of ``id``, which is then not read.  A
+        one-hot row of speaker s is exactly ``id = s``; a fade between two one-hot rows changes style over those rows."""
         mfcc = aud.to(torch.float32)
         B, _, M = mfcc.shape
         T = self.engine.latent_rows(M)
@@ -162,6 +168,8 @@ class TrainWrapper:
             ctl["seeds"] = seeds
         if anchors is not None:
             ctl["anchors"] = anchors
+        if style is not None:
+            ctl["style"] = style
         out = self.engine.body_generate(mfcc, id.to(torch.int64), noise, **ctl)
         self.last_codes, poses = out[0], out[1]
         self.last_logp = out[2] if keep_logp else None
@@ -184,7 +192,7 @@ class TrainWrapper:
         return resolve_clip_seeds(clip_seeds, B)
 
     def infer(self, aud_feat, frame, id, B, pre_latents=None, pre_audio=None, pre_pose=None, noise_fn=None,
-              temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None, anchors=None):
+              temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None, anchors=None, style=None):
         """The reference's inner call (:291-304): aud_feat [B,M,64] (time-major features of ONE chunk) ->
         (latents [B,T,2], audio [B,256,T,2], body [B,39,4T], hand [B,90,4T]).  ``pre_latents`` / ``pre_audio`` (the first
         two results of the previous chunk's call) condition the sampler on that chunk (GatedPixelCNN.generate :158-165);
@@ -194,7 +202,7 @@ class TrainWrapper:
         ``clip_seeds`` as in ``generate``; with ``pre_latents`` the chunk's draws are keyed by their absolute rows (after
         the T0 rows of the previous chunk), so a seeded clip's noise does not depend on where it is cut into chunks.
         ``anchors`` [B,T,2] cover this chunk's T rows (as in ``generate``); with ``pre_latents`` they pin rows after the
-        prefix."""
+        prefix.  ``style`` [B,T0+T,4] (or [B,4]) as in ``generate``, its rows covering the prefix and the chunk."""
         a = self.engine.audio_encode(aud_feat.transpose(1, 2).contiguous())            # [B,256,T]
         T = a.shape[2]
         label = id.reshape(-1)
@@ -205,6 +213,8 @@ class TrainWrapper:
             ctl["seeds"] = seeds
         if anchors is not None:
             ctl["anchors"] = anchors
+        if style is not None:
+            ctl["style"] = style
         if pre_latents is None:
             out = self.engine.pixelcnn_generate(a, label, noise, **ctl)
         else:
@@ -218,18 +228,26 @@ class TrainWrapper:
         hand = self.engine.vq_decode(1, latents[..., 1].contiguous())
         return latents, a.unsqueeze(-1).repeat(1, 1, 1, 2), body, hand
 
-    def _infer_continuity(self, aud_fn, id, fps, sr, B, keep_logp=False, **ctl):
+    def _infer_continuity(self, aud_fn, id, fps, sr, B, keep_logp=False, style=None, **ctl):
         """continuity=True (:244-269): a 2 s prefix, then the rest conditioned on the prefix's latents and audio.  The two
         chunks go through the audio encoder separately and are DECODED separately, so each chunk sees zero padding at the
-        2 s seam."""
+        2 s seam.  ``style`` covers the whole clip (rows T_a + T_b): chunk 0 gets rows [0, T_a), chunk 1, whose prefix is
+        chunk 0, all of them."""
         aud_feat, gap = get_mfcc_sepa(aud_fn, sr=sr, fps=fps)                 # (M0+M1, 64), M0
         feat = torch.from_numpy(np.ascontiguousarray(np.asarray(aud_feat, dtype=np.float32)))[None].repeat(B, 1, 1)   # [B,M,64]
         label = torch.tensor([0]) if id is None else id.reshape(-1).repeat(B)
+        st0 = st1 = None
+        if style is not None:
+            ta = self.engine.latent_rows(gap)
+            st1 = check_style(style, B, ta + self.engine.latent_rows(feat.shape[1] - gap), self.engine.pixelcnn_ncls)
+            st0 = st1[:, :ta]
         pre_pose = {"b": None, "h": None}
-        lat0, audio0, body_0, hand_0 = self.infer(feat[:, :gap], 0, label, B, pre_pose=pre_pose, keep_logp=keep_logp, **ctl)
+        lat0, audio0, body_0, hand_0 = self.infer(feat[:, :gap], 0, label, B, pre_pose=pre_pose, keep_logp=keep_logp,
+                                                  style=st0, **ctl)
         logp0, kept0 = self.last_logp, self.last_kept
         pre_pose["b"], pre_pose["h"] = body_0[:, :, -4:].transpose(1, 2), hand_0[:, :, -4:].transpose(1, 2)
-        lat1, _, body_1, hand_1 = self.infer(feat[:, gap:], 0, label, B, lat0, audio0, pre_pose, keep_logp=keep_logp, **ctl)
+        lat1, _, body_1, hand_1 = self.infer(feat[:, gap:], 0, label, B, lat0, audio0, pre_pose, keep_logp=keep_logp,
+                                             style=st1, **ctl)
         self.last_codes = torch.cat([lat0, lat1], 1)
         self.last_logp = torch.cat([logp0, self.last_logp], 1) if keep_logp else None
         self.last_kept = torch.cat([kept0, self.last_kept], 1) if kept0 is not None else None

@@ -10,7 +10,7 @@ from __future__ import annotations
 
 import torch
 
-from .engine import Engine, check_anchors, resolve_clip_seeds, sample_controls
+from .engine import Engine, check_anchors, check_style, resolve_clip_seeds, sample_controls
 from .nets.base import draw_sampler_noise
 
 
@@ -78,7 +78,7 @@ class WholeBody:
             self.e2 = None
 
     def generate(self, mfcc, wave, label, noise=None, stand=False, per_step_noise=True, temperature=1.0, top_k=0,
-                 keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None, anchors=None, keep_codes=False):
+                 keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None, anchors=None, keep_codes=False, style=None):
         """mfcc [B,64,M], wave [B,N] (16 kHz), label [B] on the device -> poses [B,F,265] (device).
         F = N*30//16000 face frames; the body (4*T frames) is padded/truncated to F like demo.py:207-211.
         Sampling controls of the body prior as in s2g_body_pixel.generate: ``temperature`` (0 = greedy, no noise is
@@ -88,7 +88,10 @@ class WholeBody:
         is drawn and each clip's motion depends only on its seed.  Not combinable with ``noise``.
         ``anchors`` [B,T,2] pins draws of the body prior (s2g_body_pixel.generate: a code pins, -1 samples).
         ``keep_codes`` keeps the body codes of the call, pinned and drawn, as self.last_codes [B,T,2] (None otherwise):
-        the codes a later call can anchor to."""
+        the codes a later call can anchor to.
+        ``style`` [B,T,ncls] or [B,ncls]: a speaker schedule for the body prior (s2g_body_pixel.generate), ``label`` is then
+        not read.  The face path keeps the demo's zero id (demo.py:173-181) whatever the style: the body prior is the only
+        net styled here (s2g_face.generate_ids takes a soft id for the face)."""
         B, _, M = mfcc.shape
         frame = wave.shape[1] * 30 // 16000
         T = self.e.latent_rows(M)
@@ -103,6 +106,8 @@ class WholeBody:
             noise = draw_sampler_noise(T, B, self.device, per_step=per_step_noise)
         if anchors is not None:
             ctl["anchors"] = anchors
+        if style is not None:
+            ctl["style"] = style
         idz = torch.zeros(B, 4, device=self.device)                    # demo.py:173-181: id not passed
         if self.e2 is not None and B <= self.overlap_batch:
             # small batch: sampler (on overlap_ctas SMs, launched first) and face regressor (on the free TPCs) side by side
@@ -124,7 +129,7 @@ class WholeBody:
                 self.last_kept.record_stream(cur)
             if keep_codes:
                 self.last_codes.record_stream(cur)
-            for t in (mfcc, label, noise, ctl.get("seeds"), ctl.get("anchors")):
+            for t in (mfcc, label, noise, ctl.get("seeds"), ctl.get("anchors"), ctl.get("style")):
                 if torch.is_tensor(t) and t.is_cuda:
                     t.record_stream(self._side)                          # allocated here, consumed on the side stream
             return self.e.assemble_pose(face, body, stand)
@@ -171,7 +176,7 @@ class WholeBody:
 
     def generate_sharded(self, mfcc, wave, label, rank, world, noise_full=None, seed=None, stand=False, gather=True,
                          group=None, temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None,
-                         anchors=None):
+                         anchors=None, style=None):
         """Multi-GPU form of ``generate`` whose RESULT DOES NOT DEPEND ON ``world`` (SURVEY.md §8e): the arguments are
         the FULL batch (host or device tensors, identical on every rank), the sampler noise is drawn for the full batch in
         the reference's order — ``noise_full`` [2T,B,2048], or drawn here from ``seed`` on this rank's device generator
@@ -183,7 +188,8 @@ class WholeBody:
         draws no noise at all, and the gathered result equals ``generate`` with the same seeds on one GPU.  ``seed`` keeps
         its meaning (the torch stream of the full-batch noise) and is not used with ``clip_seeds``.
         ``anchors`` [B,T,2] (as in ``generate``, for the full batch): rank r passes the rows of its shard, so the gathered
-        result equals ``generate`` with the same anchors on one GPU."""
+        result equals ``generate`` with the same anchors on one GPU.  ``style`` [B,T,ncls] or [B,ncls] (full batch, as in
+        ``generate``): rank r passes its shard's rows."""
         B, _, M = mfcc.shape
         lo, hi = shard_range(B, rank, world)
         T = self.e.latent_rows(M)
@@ -197,6 +203,8 @@ class WholeBody:
         seeds = resolve_clip_seeds(clip_seeds, B)
         if anchors is not None:
             ctl["anchors"] = check_anchors(anchors, B, T)[lo:hi]
+        if style is not None:
+            ctl["style"] = check_style(style, B, T, self.e.pixelcnn_ncls)[lo:hi]
         if seeds is not None:
             ctl["clip_seeds"] = seeds[lo:hi]
         elif noise_full is None and float(temperature) > 0:
