@@ -222,7 +222,10 @@ int ts_pixelcnn_score_styled(ts_engine* e, const float* aud, const int64_t* labe
  * (C = ts_vq_dim(which): 39 body / 90 hand, 78 / 180 for 6-D).  The indices are device data and are NOT range-checked (the
  * reference's F.embedding raises IndexError): every idx must lie in [0, num_embeddings) of the loaded codebook. */
 int ts_vq_decode(ts_engine* e, int which, const int64_t* idx, float* out, int B, int T, void* stream);
-/* VQVAE.encode, :196-199: poses [B,F,C] -> idx [B,T] int64 (T=F/4), e_out (may be NULL) [B,64,T]. */
+/* VQVAE.encode, :196-199: poses [B,F,C] -> idx [B,T] int64 (T=F/4), e_out (may be NULL) [B,64,T].
+ * Each index is the argmin over codes n of the fp32 distance (|z|^2 + |e_n|^2) - 2 z.e_n with torch.argmin's rule: the
+ * lowest code among equal distances, and a latent row with a NaN distance gets the first such code, as torch.argmin
+ * does.  Every index lies in [0, num_embeddings) whatever the poses hold. */
 int ts_vq_encode(ts_engine* e, int which, const float* poses, int64_t* idx, float* e_out, int B, int F,
                  void* stream);
 
@@ -239,7 +242,8 @@ int ts_face_forward(ts_engine* e, const float* wave, const float* id, float* out
  * reference forms them, accumulated in fp64; clip_out is fp64.
  *
  * VQVAE of s2g_body_vq.vq_train + get_loss (nets/smplx_body_vq.py:155-206) in eval mode: poses [B,F,C] (C = ts_vq_dim)
- * -> encoder + argmin (idx_out [B,T], T = F/4, bit-identical to ts_vq_encode) -> decoder on the quantised embeddings
+ * -> encoder + argmin (idx_out [B,T], T = F/4, bit-identical to ts_vq_encode, whose argmin rule applies: a latent row
+ * with a NaN distance gets the first such code, as torch.argmin does) -> decoder on the quantised embeddings
  * (recon_out, may be NULL, [B,F,C], bit-identical to ts_vq_decode of those indices, transposed) and per clip
  * clip_out [B,3] = { sum |recon - gt| over (F,C), sum |d recon - d gt| over (F-1,C) (d = frame-to-frame difference),
  * sum ||z - e[idx]||^2 over the T latent rows (z = encoder output before quantisation) }.
@@ -412,6 +416,51 @@ int ts_debug_attention(ts_engine* e, const ts_debug_att* a, const float* qkv, fl
  * The engine's ts_set_tensor_cores setting is unchanged afterwards. */
 int ts_debug_posconv(ts_engine* e, int mode, const float* x, const float* W_host, const float* bias_host, float* y, int B,
                      int T, void* stream);
+/* The four debug entries below share the conventions of the three above: sizes and pointers are checked before any launch
+ * (TS_ERR_INVALID), host weights are packed as the load path packs them, output buffers are copied in before the kernels
+ * and back after them, and the engine's ts_set_tensor_cores setting is unchanged afterwards.  mode is the activation
+ * format of ts_set_tensor_cores: 0 fp32, 1 the 3xTF32 (hi, lo) pair (fp32 hi with its 13 low mantissa bits clear, lo =
+ * v - hi), 6 fp32 + fp16 planes (h = fp16(v), l = fp16(v - h), uint16).
+ *
+ * The wav2vec2 feature extractor's first layer as the face forward runs it: Conv1d(1, 512, 10, stride 5, no bias) +
+ * GroupNorm(512, 512) (per clip and channel over time, biased variance, eps 1e-5, affine g / b) + erf-GELU, through
+ * conv0_stats_kernel (per-channel sums in fp64, 256 outputs per block merged with atomicAdd) and conv0_apply_kernel (the
+ * variance is E[y^2] - mean^2, clamped at 0).  wave [B,N] device fp32, N >= 10; W_host [512,1,10], g_host / b_host [512]
+ * host fp32.  The output has T0 = (N - 10) / 5 + 1 rows per clip, staged as the face forward stages it: T0 & 1 tail rows
+ * after every clip, so every buffer is [B, T0 + (T0 & 1), 512].  The tail rows are set to NaN before the launch (no kernel
+ * writes them).  Mode 0: fp32 in y; mode 1: the (hi, lo) pair in plane_hi / plane_lo (fp32), y unused; mode 6: the fp16
+ * planes only in plane_hi / plane_lo (uint16), y unused.  Samples past the last window are not read.  For T0 <= 256 a clip's
+ * statistics come from one block and repeated calls give the same bits; beyond, the order of the fp64 atomic merges
+ * varies from call to call (DESIGN.md). */
+int ts_debug_conv0_gn(ts_engine* e, int mode, const float* wave, const float* W_host, const float* g_host, const float* b_host,
+                      float* y, void* plane_hi, void* plane_lo, int B, int N, void* stream);
+/* The 50 -> 30 fps interpolation of the face forward (F.interpolate(mode='linear', align_corners=False) along time, with
+ * ATen's fp32 source positions: src = (Tin / Tout) * (t + 0.5) - 0.5 as two rounded operations, clamped at 0):
+ * x [B,Tin,C] device fp32, staged as conv6's output with Tin & 1 NaN tail rows after every clip (no read reaches them),
+ * -> y [B,Tout,C] device fp32. */
+int ts_debug_interp(ts_engine* e, const float* x, float* y, int B, int Tin, int Tout, int C, void* stream);
+/* Every LayerNorm of the face net (ln_pre_kernel, one warp per row, eps 1e-5):
+ *   y(b, t) = act( LN_C(x(b, t) + pre(b, t)) * g + b + res(b, t) ),  act 0 none, 1 ReLU,
+ * with pre (has_pre) and res (has_res) optional.  x, pre, res [B,T,C] device fp32, C in [1, 768] (the kernel holds 24
+ * values per lane; wider rows are TS_ERR_INVALID); g_host / b_host [C] host fp32.  x_split / res_split: x / res are
+ * stored split in the mode's format (modes 0 / 1: the (hi, lo) pair, which the kernel adds back exactly; mode 6: fp32 +
+ * planes, the kernel reads the fp32 copy).  The output is staged with one pad row before and after every clip, as the
+ * first_net and decoder norms stage it: every output buffer is [B, T + 2, C] and the pad rows keep what the caller put
+ * there.  y_split = 0: fp32 in y; modes 0 / 1: the (hi, lo) pair in plane_hi / plane_lo (fp32), y unused; mode 6: fp32
+ * in y and its fp16 planes in plane_hi / plane_lo (uint16).
+ * Input range: the mean is an fp32 sum of the row and the variance an fp32 sum of squared deviations, so |x| must stay
+ * below about 1e17 (the sum of squares overflows to inf beyond; the reference's Welford does not). */
+typedef struct ts_debug_ln {
+  int32_t mode, B, T, C;
+  int32_t has_pre, has_res, act;
+  int32_t x_split, res_split, y_split;
+} ts_debug_ln;
+int ts_debug_layernorm(ts_engine* e, const ts_debug_ln* a, const float* x, const float* pre, const float* res,
+                       const float* g_host, const float* b_host, float* y, void* plane_hi, void* plane_lo, void* stream);
+/* VectorQuantizerEMA.get_code_indices (the argmin of ts_vq_encode / ts_vq_score) on caller data: codebook_host
+ * [ncodes,64] host fp32 (uploaded with the squared row norms ts_load_vq computes), z [R,64] device fp32 staged as
+ * ts_vq_encode stages its latents, -> idx [R] int64 device, in [0, ncodes), torch.argmin's rule (ts_vq_encode). */
+int ts_debug_vq_argmin(ts_engine* e, const float* codebook_host, int ncodes, const float* z, int64_t* idx, int R, void* stream);
 /* Dense-contraction kernel for the face network and the VQ decoder (csrc/gemm_tc.cu):
  *   6 (default) Hopper wgmma kernel (128x128 tile) on two-term fp16-split operands (three products per MAC: fp32-grade
  *       results at twice the tf32 rate; operands must stay below 65504 in magnitude -- weights are pre-scaled per layer),

@@ -8,6 +8,7 @@
 // odd output phase) writing interleaved rows.
 #include "convstack.h"
 
+#include <climits>
 #include <cmath>
 
 namespace ts {
@@ -134,6 +135,18 @@ void pack_trunk(ts_engine* e, const Ckpt& ck, const std::string& p, int in_dim, 
   pack_stack(e, ck, p + "_enc_3.", hid, &t->s3);
 }
 
+std::vector<float> vq_code_norms(const float* cb, int ncodes) {
+  std::vector<float> EE(ncodes);
+  for (int n = 0; n < ncodes; ++n) {
+    // torch.sum(embeddings ** 2, dim=1): squares rounded to fp32 like ATen, summed exactly (double) and
+    // rounded once -- within 1 ulp of ATen's vectorised fp32 sum whatever its order
+    double s = 0.0;
+    for (int c = 0; c < 64; ++c) s += (double)(cb[(size_t)n * 64 + c] * cb[(size_t)n * 64 + c]);
+    EE[n] = (float)s;
+  }
+  return EE;
+}
+
 void pack_vq(ts_engine* e, const Ckpt& ck, VQNet* v) {
   const ts_tensor* pw = ck.get("decoder.project.weight");
   int C = (int)pw->shape[0];
@@ -144,16 +157,8 @@ void pack_vq(ts_engine* e, const Ckpt& ck, VQNet* v) {
   pack_trunk(e, ck, "encoder.", C, hid, &v->enc);
   v->pre_vq = pack_plain(e, ck, "encoder.pre_vq_conv.", hid, emb, 1);
   const float* cb = ck.f32("vq_layer.embeddings", {v->ncodes, emb});
-  std::vector<float> CB(cb, cb + (size_t)v->ncodes * emb), EE(v->ncodes);
-  for (int n = 0; n < v->ncodes; ++n) {
-    // torch.sum(embeddings ** 2, dim=1): squares rounded to fp32 like ATen, summed exactly (double) and
-    // rounded once -- within 1 ulp of ATen's vectorised fp32 sum whatever its order
-    double s = 0.0;
-    for (int c = 0; c < emb; ++c) s += (double)(cb[(size_t)n * emb + c] * cb[(size_t)n * emb + c]);
-    EE[n] = (float)s;
-  }
-  v->codebook = e->upload(CB);
-  v->ee = e->upload(EE);
+  v->codebook = e->upload(std::vector<float>(cb, cb + (size_t)v->ncodes * emb));
+  v->ee = e->upload(vq_code_norms(cb, v->ncodes));
   v->aft_vq = pack_plain(e, ck, "decoder.aft_vq_conv.", emb, hid, 1);
   pack_stack(e, ck, "decoder._dec_1.", hid, &v->d1);
   pack_up(e, ck, "decoder._up_2.", hid, hid / 2, &v->up2e, &v->up2o);
@@ -324,5 +329,25 @@ extern "C" int ts_vq_encode(ts_engine* e, int which, const float* poses, int64_t
       act_to_nct(e, q, 64, e_out, s);
     }
   });
+  TS_API_END(e)
+}
+
+extern "C" int ts_debug_vq_argmin(ts_engine* e, const float* codebook_host, int ncodes, const float* z, int64_t* idx, int R,
+                                  void* stream) {
+  TS_API_BEGIN(e)
+  require_device(e);
+  if (!codebook_host || !z || !idx) fail(TS_ERR_INVALID, "ts_debug_vq_argmin: codebook_host, z and idx are required");
+  if (ncodes < 1 || R < 1) fail(TS_ERR_INVALID, "ts_debug_vq_argmin: ncodes %d, R %d (need >= 1)", ncodes, R);
+  if ((long)ncodes * 64 > INT_MAX || (long)R * 64 > INT_MAX) fail(TS_ERR_INVALID, "ts_debug_vq_argmin: more than 2^31 - 1 elements");
+  LoadScope scope(e, "debug_vq");   // this call's codebook replaces the previous call's, packed as pack_vq packs it
+  const float* cb = e->upload(std::vector<float>(codebook_host, codebook_host + (size_t)ncodes * 64));
+  const float* ee = e->upload(vq_code_norms(codebook_host, ncodes));
+  cudaStream_t s = (cudaStream_t)stream;
+  Act3 za;
+  run_sized(e, [&] { za = new_act(e, 1, R, 64, 0, s); });   // ts_vq_encode's z: plain fp32, no pad rows
+  debug_fill(e, z, za, s);
+  vq_argmin(e, cb, ee, ncodes, za, idx, s);
+  TS_CUDA(cudaStreamSynchronize(s));
+  scope.commit();
   TS_API_END(e)
 }

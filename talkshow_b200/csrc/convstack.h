@@ -33,6 +33,8 @@ struct ConvStacks {
 
 void pack_trunk(ts_engine* e, const Ckpt& ck, const std::string& p, int in_dim, int hid, Trunk* t);
 void pack_vq(ts_engine* e, const Ckpt& ck, VQNet* v);
+// the codebook's squared row norms [ncodes] as pack_vq uploads them (cb [ncodes][64], host)
+std::vector<float> vq_code_norms(const float* cb, int ncodes);
 Act3 new_act(ts_engine* e, int B, int T, int C, int pad, cudaStream_t s, bool split = false, int tail = 0, bool planes_only = false);
 Act3 run_trunk(ts_engine* e, const Trunk& t, const Act3& x, cudaStream_t s);
 Act3 run_decoder(ts_engine* e, const VQNet& v, const Act3& q, cudaStream_t s);

@@ -147,9 +147,10 @@ __global__ void interp_kernel(Act3 in, Act3 out) {
     int c = i % out.C;
     long bt = i / out.C;
     int t = bt % out.T, b = bt / out.T;
-    // ATen's area_pixel_compute_source_index in float, as two rounded operations (no FMA contraction): at 100 s the
-    // source positions reach 5000 and a differently rounded position moves the interpolation weights by 1e-4
-    float src = __fsub_rn(__fmul_rn(scale, (float)t + 0.5f), 0.5f);
+    // ATen's area_pixel_compute_source_index in float, scale * (t + 0.5) - 0.5 rounded once (torch contracts it to an
+    // FMA): at 100 s the source positions reach 5000 and a differently rounded position moves the interpolation
+    // weights by up to 5e-4
+    float src = fmaf(scale, (float)t + 0.5f, -0.5f);
     if (src < 0.f) src = 0.f;
     int i0 = (int)src;
     if (i0 > in.T - 1) i0 = in.T - 1;
@@ -204,6 +205,24 @@ __global__ void ln_pre_kernel(Act3 x, Act3 pre, int has_pre, const float* __rest
       yr[c] = o;
     }
   }
+}
+// conv0 + GroupNorm(512, 512) + GELU of wave [B,N] into h [B,T0,512], T0 = (N - 10) / 5 + 1; stats: B * 512 * 2 doubles
+static void conv0_gn(ts_engine* e, const float* wave, const float* w, const float* g, const float* b, double* stats, int B, int N,
+                     const Act3& h, cudaStream_t s) {
+  if (e->ws.sizing) return;
+  const int T = h.T;
+  TS_CUDA(cudaMemsetAsync(stats, 0, (size_t)B * 512 * 2 * sizeof(double), s));
+  conv0_stats_kernel<<<dim3(cdiv(T, 256), B), 256, 0, s>>>(wave, w, N, T, stats);
+  conv0_apply_kernel<<<dim3(cdiv(T, 64), B), 256, 0, s>>>(wave, w, stats, g, b, N, T, h);
+  e->launches += 2;
+  TS_CUDA(cudaGetLastError());
+}
+static void interp(ts_engine* e, const Act3& x, const Act3& y, cudaStream_t s) {
+  if (e->ws.sizing) return;
+  long n = (long)y.B * y.T * y.C;
+  interp_kernel<<<(int)std::min<long>((n + 255) / 256, (long)e->sm_count * 16), 256, 0, s>>>(x, y);
+  e->launches++;
+  TS_CUDA(cudaGetLastError());
 }
 static void ln_pre(ts_engine* e, const Act3& x, const Act3* pre, const float* g, const float* b, const Act3& y, const Act3* res,
                    int act, cudaStream_t s) {
@@ -1217,13 +1236,7 @@ void face_run(ts_engine* e, const float* wave, const float* idv, float* out, int
   double* stats = e->ws.alloc<double>((size_t)B * 512 * 2);
   const bool tc = e->use_tc;   // activations stored split for the tensor-core kernel
   Act3 h = new_act(e, B, T, 512, 0, s, tc, T & 1, true);     // rows per batch even for the stride-2 convs; read by tensor-core convs only
-  if (!e->ws.sizing) {
-    TS_CUDA(cudaMemsetAsync(stats, 0, (size_t)B * 512 * 2 * sizeof(double), s));
-    conv0_stats_kernel<<<dim3(cdiv(T, 256), B), 256, 0, s>>>(wave, F.conv0_w, N, T, stats);
-    conv0_apply_kernel<<<dim3(cdiv(T, 64), B), 256, 0, s>>>(wave, F.conv0_w, stats, F.gn_g, F.gn_b, N, T, h);
-    e->launches += 2;
-    TS_CUDA(cudaGetLastError());
-  }
+  conv0_gn(e, wave, F.conv0_w, F.gn_g, F.gn_b, stats, B, N, h, s);
   for (int i = 1; i < 7; ++i) {
     int To = (T - W2V_K[i]) / W2V_S[i] + 1;
     Act3 y = new_act(e, B, To, 512, 0, s, tc && i < 6, To & 1, true);   // conv6 output feeds the interpolation: plain
@@ -1233,12 +1246,7 @@ void face_run(ts_engine* e, const float* wave, const float* idv, float* out, int
   }
   // ---- 50 -> 30 fps interpolation, feature projection ------------------------------------------
   Act3 hi = new_act(e, B, frame, 512, 0, s);
-  if (!e->ws.sizing) {
-    long n = (long)B * frame * 512;
-    interp_kernel<<<(int)std::min<long>((n + 255) / 256, (long)e->sm_count * 16), 256, 0, s>>>(h, hi);
-    e->launches++;
-    TS_CUDA(cudaGetLastError());
-  }
+  interp(e, h, hi, s);
   Act3 hn = new_act(e, B, frame, 512, 0, s, tc);
   ln_pre(e, hi, nullptr, F.fp_ln_g, F.fp_ln_b, hn, nullptr, ACT_NONE, s);
   Act3 x = new_act(e, B, frame, 768, 64, s);            // padded for the k=128 positional conv (FFMA kernel: plain)
@@ -1485,6 +1493,97 @@ extern "C" int ts_debug_posconv(ts_engine* e, int mode, const float* x, const fl
   debug_planes(ya, y, nullptr, nullptr, false, s);
   posconv(e, L, w16, unscale, xa, ya, s);
   debug_planes(ya, y, nullptr, nullptr, true, s);
+  TS_CUDA(cudaStreamSynchronize(s));
+  scope.commit();
+  TS_API_END(e)
+}
+
+extern "C" int ts_debug_conv0_gn(ts_engine* e, int mode, const float* wave, const float* W_host, const float* g_host, const float* b_host,
+                                 float* y, void* plane_hi, void* plane_lo, int B, int N, void* stream) {
+  TS_API_BEGIN(e)
+  require_device(e);
+  if (!wave || !W_host || !g_host || !b_host) fail(TS_ERR_INVALID, "ts_debug_conv0_gn: wave, W_host, g_host and b_host are required");
+  if (mode != 0 && mode != 1 && mode != 6) fail(TS_ERR_INVALID, "ts_debug_conv0_gn: mode %d (0 fp32, 1 3xTF32 pair, 6 fp16 planes)", mode);
+  if (B < 1 || N < 10) fail(TS_ERR_INVALID, "ts_debug_conv0_gn: B %d, N %d (need B >= 1, N >= 10)", B, N);
+  const int T = (N - 10) / 5 + 1;
+  if ((long)B * (T + 1) > INT_MAX / 512) fail(TS_ERR_INVALID, "ts_debug_conv0_gn: more than 2^31 - 1 output elements");
+  if (mode == 0 ? !y : (!plane_hi || !plane_lo))
+    fail(TS_ERR_INVALID, "ts_debug_conv0_gn: mode %d needs %s", mode, mode == 0 ? "y" : "plane_hi and plane_lo");
+  LoadScope scope(e, "debug_conv0");   // this call's weights replace the previous call's
+  const float* w = up(e, W_host, 5120);
+  const float* g = up(e, g_host, 512);
+  const float* b = up(e, b_host, 512);
+  TcModeGuard guard(e, mode);
+  cudaStream_t s = (cudaStream_t)stream;
+  double* stats = nullptr;
+  Act3 h;
+  run_sized(e, [&] {
+    stats = e->ws.alloc<double>((size_t)B * 512 * 2);
+    h = new_act(e, B, T, 512, 0, s, mode != 0, T & 1, true);   // face_run's h
+  });
+  debug_planes(h, y, plane_hi, plane_lo, false, s);
+  debug_fill(e, nullptr, h, s);   // NaN tail rows: nothing may write them
+  conv0_gn(e, wave, w, g, b, stats, B, N, h, s);
+  debug_planes(h, y, plane_hi, plane_lo, true, s);
+  TS_CUDA(cudaStreamSynchronize(s));
+  scope.commit();
+  TS_API_END(e)
+}
+
+extern "C" int ts_debug_interp(ts_engine* e, const float* x, float* y, int B, int Tin, int Tout, int C, void* stream) {
+  TS_API_BEGIN(e)
+  require_device(e);
+  if (!x || !y) fail(TS_ERR_INVALID, "ts_debug_interp: x and y are required");
+  if (B < 1 || Tin < 1 || Tout < 1 || C < 1) fail(TS_ERR_INVALID, "ts_debug_interp: B %d, Tin %d, Tout %d, C %d (need >= 1)", B, Tin, Tout, C);
+  if ((long)B * (Tin + 1) * C > INT_MAX || (long)B * Tout * C > INT_MAX) fail(TS_ERR_INVALID, "ts_debug_interp: more than 2^31 - 1 elements");
+  cudaStream_t s = (cudaStream_t)stream;
+  Act3 xa, ya;
+  run_sized(e, [&] {
+    xa = new_act(e, B, Tin, C, 0, s, false, Tin & 1);   // conv6's output: plain, Tin & 1 tail rows
+    ya = new_act(e, B, Tout, C, 0, s);
+  });
+  debug_fill(e, x, xa, s);
+  debug_planes(ya, y, nullptr, nullptr, false, s);
+  interp(e, xa, ya, s);
+  debug_planes(ya, y, nullptr, nullptr, true, s);
+  TS_CUDA(cudaStreamSynchronize(s));
+  TS_API_END(e)
+}
+
+extern "C" int ts_debug_layernorm(ts_engine* e, const ts_debug_ln* a, const float* x, const float* pre, const float* res,
+                                  const float* g_host, const float* b_host, float* y, void* plane_hi, void* plane_lo, void* stream) {
+  TS_API_BEGIN(e)
+  require_device(e);
+  if (!a || !x || !g_host || !b_host) fail(TS_ERR_INVALID, "ts_debug_layernorm: a, x, g_host and b_host are required");
+  const ts_debug_ln d = *a;
+  if (d.mode != 0 && d.mode != 1 && d.mode != 6) fail(TS_ERR_INVALID, "ts_debug_layernorm: mode %d (0 fp32, 1 3xTF32 pair, 6 fp16 planes)", d.mode);
+  if (d.B < 1 || d.T < 1 || d.C < 1) fail(TS_ERR_INVALID, "ts_debug_layernorm: B %d, T %d, C %d (need >= 1)", d.B, d.T, d.C);
+  if (d.C > 768) fail(TS_ERR_INVALID, "ts_debug_layernorm: width %d > 768", d.C);
+  if ((long)d.B * (d.T + 2) * d.C > INT_MAX) fail(TS_ERR_INVALID, "ts_debug_layernorm: more than 2^31 - 1 elements");
+  if (d.act != ACT_NONE && d.act != ACT_RELU) fail(TS_ERR_INVALID, "ts_debug_layernorm: act %d (0 none, 1 ReLU)", d.act);
+  if ((d.has_pre && !pre) || (d.has_res && !res)) fail(TS_ERR_INVALID, "ts_debug_layernorm: has_pre / has_res need pre / res");
+  const bool y_pair = d.y_split && d.mode != 6;   // (hi, lo) planes, no fp32 copy
+  if ((!y_pair && !y) || (d.y_split && (!plane_hi || !plane_lo)))
+    fail(TS_ERR_INVALID, "ts_debug_layernorm: y_split %d in mode %d needs %s", d.y_split, d.mode,
+         !d.y_split ? "y" : y_pair ? "plane_hi and plane_lo" : "y, plane_hi and plane_lo");
+  LoadScope scope(e, "debug_ln");   // this call's weights replace the previous call's
+  const float* g = up(e, g_host, d.C);
+  const float* b = up(e, b_host, d.C);
+  TcModeGuard guard(e, d.mode);
+  cudaStream_t s = (cudaStream_t)stream;
+  Act3 xa, pa, ra, ya;
+  run_sized(e, [&] {
+    xa = new_act(e, d.B, d.T, d.C, 0, s, d.x_split != 0);
+    if (d.has_pre) pa = new_act(e, d.B, d.T, d.C, 0, s);
+    if (d.has_res) ra = new_act(e, d.B, d.T, d.C, 0, s, d.res_split != 0);
+    ya = new_act(e, d.B, d.T, d.C, 1, s, d.y_split != 0);   // one pad row around every item, as first_net / decoder outputs
+  });
+  debug_fill(e, x, xa, s);
+  if (d.has_pre) debug_fill(e, pre, pa, s);
+  if (d.has_res) debug_fill(e, res, ra, s);
+  debug_planes(ya, y, plane_hi, plane_lo, false, s);
+  ln_pre(e, xa, d.has_pre ? &pa : nullptr, g, b, ya, d.has_res ? &ra : nullptr, d.act, s);
+  debug_planes(ya, y, plane_hi, plane_lo, true, s);
   TS_CUDA(cudaStreamSynchronize(s));
   scope.commit();
   TS_API_END(e)

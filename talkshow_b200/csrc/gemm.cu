@@ -370,7 +370,16 @@ void gather_rows(ts_engine* e, const float* table, int C, const int64_t* idx, co
   TS_CUDA(cudaGetLastError());
 }
 
-// distances = sum(x^2) + sum(e^2) - 2 x.e ; argmin, first index on ties (vqvae_modules.py:311-319)
+// torch.argmin's order on (distance, code): a NaN distance beats everything, then the smaller distance, then the lower
+// code.  On non-NaN distances this is `d < bd || (d == bd && i < bi)`.
+__device__ __forceinline__ bool vq_better(float d, int i, float bd, int bi) {
+  const bool dn = d != d, bn = bd != bd;
+  if (dn != bn) return dn;
+  return (dn || d == bd) ? i < bi : d < bd;
+}
+
+// distances = sum(x^2) + sum(e^2) - 2 x.e ; argmin in torch.argmin's order (vqvae_modules.py:311-319): first index on
+// ties, the first NaN distance when there is one, so the index is in [0, ncodes) whatever the latent row holds
 __global__ void __launch_bounds__(256) vq_argmin_kernel(const float* __restrict__ cb, const float* __restrict__ ee,
                                                         int ncodes, Act3 z, int64_t* __restrict__ idx) {
   __shared__ float xs[64];
@@ -396,19 +405,19 @@ __global__ void __launch_bounds__(256) vq_argmin_kernel(const float* __restrict_
       dot = fmaf(xs[4 * c + 3], v.w, dot);
     }
     float d = (xx + ee[n]) - 2.0f * dot;
-    if (d < bd || (d == bd && n < bi)) { bd = d; bi = n; }
+    if (vq_better(d, n, bd, bi)) { bd = d; bi = n; }
   }
   for (int o = 16; o > 0; o >>= 1) {
     float od = __shfl_xor_sync(0xffffffffu, bd, o);
     int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-    if (od < bd || (od == bd && oi < bi)) { bd = od; bi = oi; }
+    if (vq_better(od, oi, bd, bi)) { bd = od; bi = oi; }
   }
   int w = threadIdx.x >> 5;
   if ((threadIdx.x & 31) == 0) { best_d[w] = bd; best_i[w] = bi; }
   __syncthreads();
   if (threadIdx.x == 0) {
     for (int i = 1; i < 8; ++i)
-      if (best_d[i] < bd || (best_d[i] == bd && best_i[i] < bi)) { bd = best_d[i]; bi = best_i[i]; }
+      if (vq_better(best_d[i], best_i[i], bd, bi)) { bd = best_d[i]; bi = best_i[i]; }
     idx[bt] = bi;
   }
 }
@@ -417,40 +426,6 @@ void vq_argmin(ts_engine* e, const float* codebook, const float* ee, int ncodes,
   if (e->ws.sizing) return;
   if (z.C != 64) fail(TS_ERR_INVALID, "vq_argmin: embedding dim %d != 64", z.C);
   vq_argmin_kernel<<<z.B * z.T, 256, 0, s>>>(codebook, ee, ncodes, z, idx);
-  e->launches++;
-  TS_CUDA(cudaGetLastError());
-}
-
-// ---- LayerNorm over channels: one warp per row ------------------------------------------------
-__global__ void layernorm_kernel(Act3 x, const float* __restrict__ g, const float* __restrict__ bta, Act3 y, Act3 res,
-                                 int has_res, int act, float eps) {
-  int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  int rows = x.B * x.T;
-  if (warp >= rows) return;
-  int b = warp / x.T, t = warp % x.T;
-  const float* xr = x.row(b, t);
-  int C = x.C;
-  float s = 0.f;
-  for (int c = lane; c < C; c += 32) s += xr[c];
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  float mean = s / C;
-  float v = 0.f;
-  for (int c = lane; c < C; c += 32) { float d = xr[c] - mean; v = fmaf(d, d, v); }
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  float rstd = rsqrtf(v / C + eps);
-  float* yr = y.row(b, t);
-  const float* rr = has_res ? res.row(b, t) : nullptr;
-  for (int c = lane; c < C; c += 32) {
-    float o = (xr[c] - mean) * rstd * g[c] + bta[c];
-    if (rr) o += rr[c];
-    yr[c] = act_apply(o, act);
-  }
-}
-void layernorm(ts_engine* e, const Act3& x, const float* g, const float* b, const Act3& y, const Act3* res, int act,
-               float eps, cudaStream_t s) {
-  if (e->ws.sizing) return;
-  int rows = x.B * x.T;
-  layernorm_kernel<<<cdiv(rows, 8), 256, 0, s>>>(x, g, b, y, res ? *res : Act3(), res ? 1 : 0, act, eps);
   e->launches++;
   TS_CUDA(cudaGetLastError());
 }

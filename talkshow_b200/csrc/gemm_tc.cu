@@ -506,7 +506,8 @@ extern "C" int ts_set_tensor_cores(ts_engine* e, int enable) {
 
 namespace ts {
 // x [B, a.T, a.C] -> rows [0, a.T) of every batch item of `a`, in a's storage format (fp32, 3xTF32 pair or fp32 + fp16
-// planes); the tail rows of every plane get NaN: no conv may read them.  Pad rows keep new_act's zeros.
+// planes); the tail rows of every plane get NaN: no conv may read them.  Pad rows keep new_act's zeros.  x = NULL: rows
+// [0, a.T) are left as they are (only the tail rows are written).
 __global__ void debug_fill_kernel(const float* __restrict__ x, Act3 a) {
   const int rows = a.T + 2 * a.pad + a.tail;
   const long n = (long)a.B * rows * a.C;
@@ -514,7 +515,10 @@ __global__ void debug_fill_kernel(const float* __restrict__ x, Act3 a) {
     const int c = (int)(i % a.C), r = (int)((i / a.C) % rows), b = (int)(i / ((long)a.C * rows));
     const int t = r - a.pad;
     float v;
-    if (t >= 0 && t < a.T) v = x[((long)b * a.T + t) * a.C + c];
+    if (t >= 0 && t < a.T) {
+      if (!x) continue;
+      v = x[((long)b * a.T + t) * a.C + c];
+    }
     else if (r >= a.T + 2 * a.pad) v = __int_as_float(0x7fffffff);
     else continue;
     if (a.lo) {

@@ -75,9 +75,6 @@ void gather_rows(ts_engine* e, const float* table, int C, const int64_t* idx, co
 // VectorQuantizerEMA.get_code_indices (vqvae_modules.py:311-319): z rows -> argmin index
 void vq_argmin(ts_engine* e, const float* codebook, const float* ee, int ncodes, const Act3& z, int64_t* idx,
                cudaStream_t s);
-// row-wise LayerNorm over C, y = LN(x)*g+b (+res) then act; x,y,res channel-last with C channels
-void layernorm(ts_engine* e, const Act3& x, const float* g, const float* b, const Act3& y, const Act3* res, int act,
-               float eps, cudaStream_t s);
 
 // ---- tensor-core path (gemm_tc.cu): Hopper wgmma on fp16-split or 3xTF32 operands, TMA-staged ------
 bool tc_conv_supported(ts_engine* e, const Layer& L, const Act3& x, int stride, int pd);
@@ -95,7 +92,8 @@ void conv_auto(ts_engine* e, const Layer& L, const Act3& x, int k, int stride, i
 
 // ---- debug entry points (ts_debug_*): one kernel on caller data, staged as the nets stage it ----------------------------
 // x [B, a.T, a.C] -> rows [0, a.T) of every item of `a`, in a's storage format (fp32, 3xTF32 pair or fp32 + fp16 planes);
-// the tail rows of every plane get NaN (no kernel may read them), pad rows keep new_act's zeros
+// the tail rows of every plane get NaN (no kernel may read them), pad rows keep new_act's zeros; x = NULL writes the tail
+// rows only
 void debug_fill(ts_engine* e, const float* x, const Act3& a, cudaStream_t s);
 // copy the caller's output buffers into a's planes (back = false) or a's planes out to them (back = true): y <-> a.p, or
 // plane_hi / plane_lo <-> the (hi, lo) pair (a.p, a.lo) or the fp16 planes (a.h16, a.l16) beside y <-> a.p

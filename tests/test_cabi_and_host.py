@@ -70,7 +70,9 @@ def test_host_only_engine_rejects_execution_and_bad_checkpoints():
                        ("ts_assemble_pose", (h, n, n, n, 1, 4, 4, 0, n)), ("ts_rot6d_to_axis_angle", (h, n, n, 4, n)),
                        ("ts_pixelcnn_generate", (h, n, n, n, n, n, 1, 2, n, 0, n)), ("ts_pixelcnn_timing", (h, 1)), ("ts_mfcc", (h, n, n, 1, 16000, 16000, n)),
                        ("ts_debug_conv1d", (h, n, n, n, n, n, n, n, n, n)), ("ts_debug_attention", (h, n, n, n, n, n, n)),
-                       ("ts_debug_posconv", (h, 6, n, n, n, n, 1, 8, n))):
+                       ("ts_debug_posconv", (h, 6, n, n, n, n, 1, 8, n)),
+                       ("ts_debug_conv0_gn", (h, 6, n, n, n, n, n, n, n, 1, 400, n)), ("ts_debug_interp", (h, n, n, 1, 8, 5, 4, n)),
+                       ("ts_debug_layernorm", (h, n, n, n, n, n, n, n, n, n, n)), ("ts_debug_vq_argmin", (h, n, 8, n, n, 4, n))):
         assert getattr(L, name)(*args) != 0 and b"host-only" in L.ts_last_error(h), name
     assert L.ts_set_vq_parallel(h, -1) != 0 and L.ts_set_vq_parallel(h, 16) == 0 and L.ts_set_pixelcnn_mode(h, 7) != 0
     with pytest.raises(ValueError):
