@@ -203,6 +203,30 @@ int ts_pixelcnn_sample_styled(ts_engine* e, const float* aud, const int64_t* lab
                               const float* noise, const int64_t* seeds, const int64_t* anchors, int64_t* idx_out,
                               float* logits_out, int B, int T, const int64_t* pre_latents, int T0, const ts_sample_ctl* ctl,
                               void* stream);
+/* ---- per-clip sampling controls: each clip of a batch with its own temperature, top_k, top_p and min_p ----------------
+ * One entry per clip: the four controls of ts_sample_ctl, with their ranges and their meaning. */
+typedef struct ts_clip_ctl {
+  float temperature;   /* >= 0, finite; 0 = greedy */
+  int32_t top_k;       /* [0, 2048]; 0 or 2048 = off */
+  float top_p;         /* (0, 1]; 1 = off */
+  float min_p;         /* [0, 1]; 0 = off */
+} ts_clip_ctl;
+/* ts_pixelcnn_sample_styled where clip b draws with clip_ctl[b] in place of ctl's four controls.
+ *  - clip_ctl [B] is HOST memory.  Every entry is checked on the host with the rules of ts_sample_ctl before any launch
+ *    (TS_ERR_INVALID, the message names the clip), then the entries are copied to engine-owned device memory on `stream`
+ *    (the caller's array may be reused when the call returns; no synchronisation).
+ *  - ctl (may be NULL) supplies logp_out and kept_out only; its temperature, top_k, top_p and min_p are not read.
+ *  - Clip b's codes, logp_out and kept_out equal bit for bit those of clip b run alone through ts_pixelcnn_sample_styled
+ *    with ctl = clip_ctl[b] (the same noise column or seed, anchors, style rows and pre_latents): the logits of a clip do
+ *    not depend on the batch, and the draw reads only the clip's own controls.
+ *  - A greedy clip (temperature 0) reads no noise; noise keeps its [2T,B,2048] shape.  Exactly one of noise and seeds
+ *    must be given when any clip has temperature > 0; neither is needed when every clip is greedy.
+ * The call runs the kernels and launches of ts_pixelcnn_sample_styled (no extra kernel: one host-to-device copy).
+ * clip_ctl = NULL: the call equals ts_pixelcnn_sample_styled with the same arguments, bit for bit and with its launches. */
+int ts_pixelcnn_sample_clips(ts_engine* e, const float* aud, const int64_t* label, const float* style, int ncls,
+                             const float* noise, const int64_t* seeds, const int64_t* anchors, int64_t* idx_out,
+                             float* logits_out, int B, int T, const int64_t* pre_latents, int T0, const ts_sample_ctl* ctl,
+                             const ts_clip_ctl* clip_ctl, void* stream);
 /* GatedPixelCNN.forward (teacher forced), :130-150, for rows [0,T): logits_out [B,2048,T,2]. */
 int ts_pixelcnn_logits(ts_engine* e, const float* aud, const int64_t* label, const int64_t* codes,
                        float* logits_out, int B, int T, void* stream);
@@ -294,6 +318,11 @@ int ts_body_sample_anchored(ts_engine* e, const float* mfcc, const int64_t* labe
 int ts_body_sample_styled(ts_engine* e, const float* mfcc, const int64_t* label, const float* style, int ncls,
                           const float* noise, const int64_t* seeds, const int64_t* anchors, int64_t* codes, float* poses,
                           int B, int M, const ts_sample_ctl* ctl, void* stream);
+/* ts_body_sample_styled with the per-clip controls of ts_pixelcnn_sample_clips (clip_ctl [B] in host memory, ctl for
+ * logp_out / kept_out only); the poses decode each clip's codes.  clip_ctl = NULL equals ts_body_sample_styled. */
+int ts_body_sample_clips(ts_engine* e, const float* mfcc, const int64_t* label, const float* style, int ncls,
+                         const float* noise, const int64_t* seeds, const int64_t* anchors, int64_t* codes, float* poses,
+                         int B, int M, const ts_sample_ctl* ctl, const ts_clip_ctl* clip_ctl, void* stream);
 
 /* Audio front-end of get_mfcc_ta, data_utils/utils.py:148-177 (SURVEY.md §8f-1): wave [B,N] mono at
  * `sr` Hz -> torchaudio Resample(sr, 22000) -> MFCC(64 coefficients, n_fft 2048, hop 734 = 30 fps, 256 HTK

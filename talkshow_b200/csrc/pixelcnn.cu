@@ -481,7 +481,32 @@ struct PixArgs {
   const float* style;
   const float* cls_w;
   int ncls;
+  // per-clip controls (ts_pixelcnn_sample_clips), read by the WARP instantiations only: [B] (device), indexed by the
+  // global clip index; or null (the scalar controls above)
+  const ts_clip_ctl* clip_ctl;
 };
+
+// The sampling controls of clip m (global index): its entry of A.clip_ctl, else the call's scalar controls.  Every draw
+// of one clip runs in one CTA, so the value is uniform over the threads that call draw_controlled together.
+static_assert(sizeof(ts_clip_ctl) == 16, "ts_clip_ctl is read as one 16-byte load");
+struct DrawCtl {
+  float temperature;
+  int top_k;
+  float top_p, min_p;
+};
+template <class Args>
+__device__ __forceinline__ DrawCtl draw_ctl(const Args& A, int m) {
+  if (A.clip_ctl) {
+    const int4 v = __ldg(reinterpret_cast<const int4*>(A.clip_ctl) + m);
+    return {__int_as_float(v.x), v.y, __int_as_float(v.z), __int_as_float(v.w)};
+  }
+  return {A.temperature, A.top_k, A.top_p, A.min_p};
+}
+// The temperature of clip m alone (the noise prefetch before the barrier wait: a greedy clip reads no noise).
+template <class Args>
+__device__ __forceinline__ float draw_temperature(const Args& A, int m) {
+  return A.clip_ctl ? __ldg(&A.clip_ctl[m].temperature) : A.temperature;
+}
 
 // The speaker weights of row r of clip m (global index) under A.style, or null for a padding sample (m >= B).
 template <class Args>
@@ -1404,8 +1429,9 @@ __device__ void run_sample_task(const PixTask& t, const PixArgs& A, int r, int m
         code = pin;
         draw_pinned(l, code, red, A.logp_out ? A.logp_out + at : nullptr, A.kept_out ? A.kept_out + at : nullptr, CtaBar());
       } else {
+        const DrawCtl dc = draw_ctl(A, m);   // clip m's controls: the whole CTA serves clip m
         float qv[8];
-        if (A.temperature > 0.f) {
+        if (dc.temperature > 0.f) {
           if (QPRE) {
 #pragma unroll
             for (int j = 0; j < 8; ++j) qv[j] = qpre[j];
@@ -1413,7 +1439,7 @@ __device__ void run_sample_task(const PixTask& t, const PixArgs& A, int r, int m
             draw_noise(A, r, c, m, qv);
           }
         }
-        code = draw_controlled(l, qv, A.temperature, A.top_k, A.top_p, A.min_p, red, A.logp_out ? A.logp_out + at : nullptr,
+        code = draw_controlled(l, qv, dc.temperature, dc.top_k, dc.top_p, dc.min_p, red, A.logp_out ? A.logp_out + at : nullptr,
                                A.kept_out ? A.kept_out + at : nullptr, CtaBar());
       }
     } else {
@@ -1573,7 +1599,7 @@ __global__ void __launch_bounds__(PIX_THREADS, 1) pixelcnn_kernel(PixArgs A, int
     // the sampler noise of this position is an input of the call (or, seeded, a function of the seed and the position):
     // loaded / computed before the barrier wait, so it overlaps the wait
     float qpre[8];
-    if (active && t.epi == EPI_SAMPLE && cta < A.B && r >= A.T0 && (!WARP || A.temperature > 0.f))   // greedy: no noise
+    if (active && t.epi == EPI_SAMPLE && cta < A.B && r >= A.T0 && (!WARP || draw_temperature(A, cta) > 0.f))   // greedy: no noise
       draw_noise(A, r, t.col, cta, qpre);
     if (has_w) { mbar_wait(&bars[buf], uses[buf] & 1u); uses[buf]++; }
     unsigned long long* tr = nullptr;
@@ -1643,7 +1669,7 @@ __global__ void logits_to_ref_kernel(const float* __restrict__ in, float* __rest
 static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t* label, const float* noise, int noise_B,
                            int64_t* idx_out, float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s,
                            bool logits_all, const SampleCtl* ctl, const int64_t* seeds, const int64_t* anchors,
-                           const float* style) {
+                           const float* style, const ts_clip_ctl* clip_ctl) {
   PixelPlan* P = e->pix;
   Plan3* Q = (Plan3*)P->p3;
   const int Ttot = T0 + T, D = P->D;
@@ -1671,7 +1697,7 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
 
   if (v3) {   // cluster-resident executor (pixelcnn3.inc): any batch size, clusters of 16 CTAs per 4 / 8 samples
     launch_pixelcnn3(e, P, Q, audv, audh, label, noise, idx_out, logits_out, B, T0, Ttot, pre, logits_all, arena3, MB3, s, ctl, seeds,
-                     anchors, style);
+                     anchors, style, clip_ctl);
     return;
   }
   if (B > PIX_MB)
@@ -1705,6 +1731,7 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
   A.seeds = seeds;
   A.anchors = anchors;
   A.style = style; A.cls_w = P->d_cls; A.ncls = P->nclasses;
+  A.clip_ctl = clip_ctl;
   if (e->pixel_mode == 0) {
     // A/B switch: 0 = burst loads + scalar FFMA, 4 = pipelined loads + scalar FFMA, 5 (default) = pipelined loads + paired FMAs (fma2)
     static const int pipe = getenv("TS_PIX_PIPE") ? atoi(getenv("TS_PIX_PIPE")) : 5;
@@ -1778,13 +1805,19 @@ void pixel_destroy(ts_engine* e) {
 
 void pixelcnn_generate_act(ts_engine* e, const Act3& aud, const int64_t* label, const float* noise, int64_t* idx_out,
                            float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s, bool logits_all,
-                           const SampleCtl* ctl, const int64_t* seeds, const int64_t* anchors, const float* style) {
+                           const SampleCtl* ctl, const int64_t* seeds, const int64_t* anchors, const float* style,
+                           const ts_clip_ctl* clip_ctl) {
   if (!e->pix) fail(TS_ERR_NOT_LOADED, "pixelcnn weights not loaded");
-  // an anchored or styled call always runs the WARP kernels; without controls at temperature 1, top_k 0 (the default
-  // draw's bits)
+  // an anchored, styled or per-clip call always runs the WARP kernels; without controls at temperature 1, top_k 0 (the
+  // default draw's bits)
   const SampleCtl dflt;
-  if ((anchors || style) && !ctl) ctl = &dflt;
-  generate_chunk(e, aud, 0, label, noise, B, idx_out, logits_out, B, T, pre, T0, s, logits_all, ctl, seeds, anchors, style);
+  if ((anchors || style || clip_ctl) && !ctl) ctl = &dflt;
+  // per-clip controls: host entries (validated by the caller) -> workspace, in stream order before the sampler reads them
+  ts_clip_ctl* dclip = clip_ctl ? e->ws.alloc<ts_clip_ctl>((size_t)B) : nullptr;
+  if (dclip && !e->ws.sizing)
+    TS_CUDA(cudaMemcpyAsync(dclip, clip_ctl, (size_t)B * sizeof(ts_clip_ctl), cudaMemcpyHostToDevice, s));
+  generate_chunk(e, aud, 0, label, noise, B, idx_out, logits_out, B, T, pre, T0, s, logits_all, ctl, seeds, anchors, style,
+                 dclip);
 }
 
 void check_style(const ts_engine* e, const int64_t* label, const float* style, int ncls, const char* who) {
@@ -1813,6 +1846,22 @@ void check_anchored_source(const SampleCtl* ctl, const float* noise, const int64
   if (!greedy && (noise != nullptr) == (seeds != nullptr))
     fail(TS_ERR_INVALID, "%s: noise=%p seeds=%p (give exactly one; only greedy decoding runs without)", who, (const void*)noise,
          (const void*)seeds);
+}
+
+void check_clip_ctl(const ts_clip_ctl* clip_ctl, int B, const float* noise, const int64_t* seeds, const char* who) {
+  bool sampled = false;
+  for (int b = 0; b < B; ++b) {
+    const ts_clip_ctl& c = clip_ctl[b];
+    if (!std::isfinite(c.temperature) || c.temperature < 0.f)
+      fail(TS_ERR_INVALID, "%s: clip %d: temperature %g (must be finite and >= 0)", who, b, (double)c.temperature);
+    if (c.top_k < 0 || c.top_k > PIX_NCODE) fail(TS_ERR_INVALID, "%s: clip %d: top_k %d outside [0, %d]", who, b, c.top_k, PIX_NCODE);
+    if (!(c.top_p > 0.f && c.top_p <= 1.f)) fail(TS_ERR_INVALID, "%s: clip %d: top_p %g outside (0, 1]", who, b, (double)c.top_p);
+    if (!(c.min_p >= 0.f && c.min_p <= 1.f)) fail(TS_ERR_INVALID, "%s: clip %d: min_p %g outside [0, 1]", who, b, (double)c.min_p);
+    sampled = sampled || c.temperature > 0.f;
+  }
+  if (sampled && (noise != nullptr) == (seeds != nullptr))
+    fail(TS_ERR_INVALID, "%s: noise=%p seeds=%p (give exactly one; only a batch of greedy clips runs without)", who,
+         (const void*)noise, (const void*)seeds);
 }
 
 SampleCtl sample_ctl_of(const ts_sample_ctl* c) {
@@ -1955,15 +2004,16 @@ static void check_pix(ts_engine* e, int B, int T) {
 static void pixelcnn_generate_call(ts_engine* e, const float* aud, const int64_t* label, const float* noise, int64_t* idx_out,
                                    float* logits_out, int B, int T, const int64_t* pre_latents, int T0, void* stream,
                                    const SampleCtl* ctl, const int64_t* seeds = nullptr, const int64_t* anchors = nullptr,
-                                   const float* style = nullptr) {
+                                   const float* style = nullptr, const ts_clip_ctl* clip_ctl = nullptr) {
   check_pix(e, B, T);
   if (T0 < 0 || (T0 > 0 && !pre_latents)) fail(TS_ERR_INVALID, "pixelcnn: T0=%d without pre_latents", T0);
-  if (ctl) check_sample_ctl(*ctl, noise, seeds);
+  if (ctl && !clip_ctl) check_sample_ctl(*ctl, noise, seeds);
   cudaStream_t s = (cudaStream_t)stream;
   auto body = [&] {
     Act3 a = new_act(e, B, T0 + T, 256, 0, s);
     nct_to_act(e, aud, 256, a, s);
-    pixelcnn_generate_act(e, a, label, noise, idx_out, logits_out, B, T, pre_latents, T0, s, false, ctl, seeds, anchors, style);
+    pixelcnn_generate_act(e, a, label, noise, idx_out, logits_out, B, T, pre_latents, T0, s, false, ctl, seeds, anchors, style,
+                          clip_ctl);
   };
   e->ws.begin_sizing(); body();
   size_t need = e->ws.need;
@@ -2062,6 +2112,26 @@ extern "C" int ts_pixelcnn_sample_styled(ts_engine* e, const float* aud, const i
   check_anchored_source(ctl ? &c : nullptr, noise, seeds, "ts_pixelcnn_sample_styled");
   pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, ctl ? &c : nullptr, seeds,
                          anchors, style);
+  TS_API_END(e)
+}
+
+// clip_ctl [B] (host): each clip's temperature, top_k, top_p and min_p, validated here and copied to the workspace on the
+// call's stream; ctl (may be NULL) gives logp_out / kept_out only.  NULL: ts_pixelcnn_sample_styled with its launches and bits.
+extern "C" int ts_pixelcnn_sample_clips(ts_engine* e, const float* aud, const int64_t* label, const float* style, int ncls,
+                                        const float* noise, const int64_t* seeds, const int64_t* anchors, int64_t* idx_out,
+                                        float* logits_out, int B, int T, const int64_t* pre_latents, int T0,
+                                        const ts_sample_ctl* ctl, const ts_clip_ctl* clip_ctl, void* stream) {
+  if (!clip_ctl)
+    return ts_pixelcnn_sample_styled(e, aud, label, style, ncls, noise, seeds, anchors, idx_out, logits_out, B, T, pre_latents,
+                                     T0, ctl, stream);
+  TS_API_BEGIN(e)
+  check_pix(e, B, T);
+  check_style(e, label, style, ncls, "ts_pixelcnn_sample_clips");
+  check_clip_ctl(clip_ctl, B, noise, seeds, "ts_pixelcnn_sample_clips");
+  SampleCtl c;   // logp_out / kept_out of ctl; the draws' controls come from clip_ctl
+  if (ctl) { c.logp_out = ctl->logp_out; c.kept_out = ctl->kept_out; }
+  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, &c, seeds, anchors, style,
+                         clip_ctl);
   TS_API_END(e)
 }
 

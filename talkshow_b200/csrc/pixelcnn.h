@@ -91,11 +91,13 @@ SampleCtl sample_ctl_of(const ts_sample_ctl* c);
 // draws' noise is computed from the per-clip seeds (ts_pixelcnn_sample_seeded) and `noise` is not read.  anchors
 // [B,T,2] (device): the pinned draws of ts_pixelcnn_sample_anchored; the call then runs the WARP kernels, at the default
 // controls when ctl is null.  style [B,T0+T,ncls] (device): the speaker schedule of ts_pixelcnn_sample_styled (label
-// unread), likewise on the WARP kernels.
+// unread), likewise on the WARP kernels.  clip_ctl [B] (HOST, validated with check_clip_ctl): the per-clip controls of
+// ts_pixelcnn_sample_clips, copied to the workspace on s; each clip draws with its entry in place of ctl's four controls.
 void pixelcnn_generate_act(ts_engine* e, const Act3& aud, const int64_t* label, const float* noise, int64_t* idx_out,
                            float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s,
                            bool logits_all = false, const SampleCtl* ctl = nullptr, const int64_t* seeds = nullptr,
-                           const int64_t* anchors = nullptr, const float* style = nullptr);
+                           const int64_t* anchors = nullptr, const float* style = nullptr,
+                           const ts_clip_ctl* clip_ctl = nullptr);
 // The class terms of gate channel q (tanh half) and D + q (sigmoid half) under one row's speaker weights w[0..ncls)
 // (ts_pixelcnn_sample_styled): acc = w0 E[0][ch], then acc + w_s E[s][ch] for s = 1 .. ncls-1, every product and sum
 // rounded to fp32 without contraction.  tab: one layer's class_cond_embedding [ncls][2D]; w null (a padding sample of the
@@ -120,6 +122,9 @@ constexpr int PIX_MAXCLS = 16;
 void check_style(const ts_engine* e, const int64_t* label, const float* style, int ncls, const char* who);
 // The noise source of an anchored call (TS_ERR_INVALID): exactly one of noise and seeds unless ctl is greedy.
 void check_anchored_source(const SampleCtl* ctl, const float* noise, const int64_t* seeds, const char* who);
+// The per-clip controls of ts_pixelcnn_sample_clips (TS_ERR_INVALID, naming the clip): every entry by the rules of
+// check_sample_ctl, and exactly one of noise and seeds when any clip samples (temperature > 0).  clip_ctl: B host entries.
+void check_clip_ctl(const ts_clip_ctl* clip_ctl, int B, const float* noise, const int64_t* seeds, const char* who);
 // idx [B,T,2] -> idx_c [2][B][T]; optionally copies idx to codes_out
 void split_codes(ts_engine* e, const int64_t* idx, int64_t* idx_c, int B, int T, int64_t* codes_out, cudaStream_t s);
 void pixel_destroy(ts_engine* e);

@@ -43,7 +43,13 @@ def sample_controls(temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=
     """Validated keyword arguments of ``Engine.pixelcnn_generate`` / ``body_generate`` for these controls; empty at the
     defaults, so that those calls keep the default entry points (ts_pixelcnn_generate / ts_body_generate).  ``top_p``,
     ``min_p`` and ``want_kept`` appear only when nucleus or min-p truncation is on; the keep-set sizes are then asked for
-    together with the log-likelihoods."""
+    together with the log-likelihoods.  Per-clip controls (``check_clip_controls``) give all four as float32 / int32
+    arrays [B], with ``want_kept`` when any clip truncates by top_p or min_p."""
+    if per_clip(temperature, top_k, top_p, min_p):
+        cc = check_clip_controls(temperature, top_k, top_p, min_p)
+        nucleus = bool((cc["top_p"] < 1.0).any() or (cc["min_p"] > 0.0).any())
+        return dict(temperature=cc["temperature"], top_k=cc["top_k"], want_logp=bool(keep_logp), top_p=cc["top_p"],
+                    min_p=cc["min_p"], want_kept=bool(keep_logp) and nucleus)
     check_sample_controls(temperature, top_k, top_p, min_p)
     nucleus = float(top_p) < 1.0 or float(min_p) > 0.0
     if float(temperature) == 1.0 and not top_k and not keep_logp and not nucleus:
@@ -52,6 +58,73 @@ def sample_controls(temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=
     if nucleus:
         ctl.update(top_p=top_p, min_p=min_p, want_kept=bool(keep_logp))
     return ctl
+
+
+# one entry of the per-clip controls (include/talkshow_b200.h ts_clip_ctl)
+CLIP_CTL = np.dtype([("temperature", "<f4"), ("top_k", "<i4"), ("top_p", "<f4"), ("min_p", "<f4")])
+
+
+def _is_per_clip(v):
+    """A control given per clip: a list / tuple, or a numpy array or tensor with a dimension (a 0-d one is a scalar)."""
+    if torch.is_tensor(v) or isinstance(v, np.ndarray):
+        return v.ndim > 0
+    return isinstance(v, (list, tuple))
+
+
+def per_clip(temperature, top_k, top_p=1.0, min_p=0.0):
+    """True when any of the four sampling controls is given per clip (``check_clip_controls``)."""
+    return any(_is_per_clip(v) for v in (temperature, top_k, top_p, min_p))
+
+
+def check_clip_controls(temperature, top_k, top_p=1.0, min_p=0.0, B=None):
+    """Per-clip sampling controls as a host array [B] of ``CLIP_CTL`` (ts_clip_ctl).  Each control is a scalar, broadcast
+    to every clip, or a length-B sequence / 1-D numpy array / 1-D tensor; B defaults to the length of the per-clip
+    values.  Every clip's values follow ``check_sample_controls`` (fp32 rounding of top_p / min_p included) and a
+    temperature must stay finite in fp32.  A bool element, another shape or another length raises ValueError; an
+    element's error names its clip."""
+    cols = {}
+    for name, v in (("temperature", temperature), ("top_k", top_k), ("top_p", top_p), ("min_p", min_p)):
+        if not _is_per_clip(v):
+            continue
+        if torch.is_tensor(v) or isinstance(v, np.ndarray):
+            if v.ndim != 1:
+                raise ValueError("%s: per-clip values must be one-dimensional, got shape %s" % (name, tuple(v.shape)))
+            v = v.tolist()
+        v = list(v)
+        if B is None:
+            B = len(v)
+        if len(v) != B:
+            raise ValueError("%s: %d per-clip values for %d clips" % (name, len(v), B))
+        for b, x in enumerate(v):
+            if isinstance(x, bool):
+                raise ValueError("%s: clip %d: a bool is not a sampling control, got %r" % (name, b, x))
+        cols[name] = v
+    if B is None:
+        raise ValueError("check_clip_controls: no per-clip value and no batch size")
+    scalars = dict(temperature=temperature, top_k=top_k, top_p=top_p, min_p=min_p)
+    defaults = dict(temperature=1.0, top_k=0, top_p=1.0, min_p=0.0)
+    check_sample_controls(**{n: defaults[n] if n in cols else v for n, v in scalars.items()})   # the broadcast scalars
+    out = np.zeros(B, CLIP_CTL)
+    for b in range(B):
+        t, k, p, m = (cols[n][b] if n in cols else scalars[n] for n in ("temperature", "top_k", "top_p", "min_p"))
+        try:
+            check_sample_controls(t, k, p, m)
+            with np.errstate(over="ignore"):
+                t32 = np.float32(float(t))
+            if not math.isfinite(t32):
+                raise ValueError("temperature must be finite in fp32, got %r" % (t,))
+        except ValueError as ex:
+            raise ValueError("clip %d: %s" % (b, ex)) from None
+        out[b] = (float(t), int(k), float(p), float(m))
+    return out
+
+
+def sampled(temperature):
+    """True when a call with this (validated) temperature draws noise: temperature > 0, for some clip when per clip."""
+    if _is_per_clip(temperature):
+        vals = temperature.tolist() if hasattr(temperature, "tolist") else temperature
+        return any(float(t) > 0 for t in vals)
+    return float(temperature) > 0
 
 
 def _wrap64(v):
@@ -161,6 +234,17 @@ def _controlled(temperature, top_k, noise, want_logp, top_p=1.0, min_p=0.0, want
         raise ValueError("sampling at temperature %g needs the noise tensor or per-clip seeds (only greedy decoding, "
                          "temperature 0, runs without)" % float(temperature))
     return bool(sample_controls(temperature, top_k, want_logp, top_p, min_p)) or bool(want_kept)
+
+
+def _clip_source(clip, noise, seeds):
+    """Engine side of a per-clip call: the noise source rule (exactly one of noise and seeds when any clip samples)."""
+    if noise is not None and seeds is not None:
+        raise ValueError("give the sampler either noise or seeds, not both")
+    if noise is None and seeds is None and (clip["temperature"] > 0).any():
+        raise ValueError("clip %d samples at temperature %g: the call needs the noise tensor or per-clip seeds (only a "
+                         "batch of greedy clips runs without)" % (int(np.argmax(clip["temperature"] > 0)),
+                                                                  float(clip["temperature"].max())))
+    return True
 
 
 def _needs_ctl(top_p, min_p, want_kept):
@@ -362,8 +446,19 @@ class Engine:
         ``style`` (``check_style``: [B,T0+T,ncls] or [B,ncls], float) replaces the speaker label with a per-row convex
         mixture of the prior's speaker embeddings (ts_pixelcnn_sample_styled; rule in include/talkshow_b200.h).  Its rows
         cover every row the network sees, the ``pre_latents`` prefix included; ``label`` is then not read and may be None.
-        A one-hot schedule of class s draws what label s draws.  None forwards exactly what the call forwards without it."""
-        ctl = _controlled(temperature, top_k, noise, want_logp, top_p, min_p, want_kept, seeds)
+        A one-hot schedule of class s draws what label s draws.  None forwards exactly what the call forwards without it.
+
+        Per-clip controls: ``temperature``, ``top_k``, ``top_p`` and ``min_p`` each take a scalar or one value per clip
+        (a length-B sequence, 1-D numpy array or 1-D tensor; ``check_clip_controls``), a scalar among them applying to every
+        clip.  Clip b then draws exactly what it draws alone under its own values (ts_pixelcnn_sample_clips), whatever the
+        other clips' values; a greedy clip reads no noise.  Sampling takes exactly one of noise and seeds when any clip has
+        temperature > 0.  All-scalar calls forward what they forwarded before."""
+        clip = None
+        if per_clip(temperature, top_k, top_p, min_p):
+            clip = check_clip_controls(temperature, top_k, top_p, min_p, aud.shape[0])
+            ctl = _clip_source(clip, noise, seeds)
+        else:
+            ctl = _controlled(temperature, top_k, noise, want_logp, top_p, min_p, want_kept, seeds)
         aud = self._dev(aud, torch.float32)
         B = aud.shape[0]
         if label is None and style is None:
@@ -395,7 +490,14 @@ class Engine:
             kz = kept if (full or kept is None) else torch.empty(nb, T, 2, dtype=torch.int32, device=self.device)
             args = (self.h, _lib.ptr(aud[b0:b1].contiguous()), _lib.ptr(None if label is None else label[b0:b1].contiguous()), _lib.ptr(nz),
                     _lib.ptr(cz), _lib.ptr(lz), nb, T, _lib.ptr(None if pre is None else pre[b0:b1].contiguous()), T0)
-            if style is not None:
+            if clip is not None:
+                c = _ctl_struct(1.0, 0, 1.0, 0.0, pz, kz)      # logp / kept only: the draws' controls are clip[b0:b1]
+                args = args[:3] + (_lib.ptr(None if style is None else style[b0:b1]), self.pixelcnn_ncls, _lib.ptr(nz),
+                                   _lib.ptr(None if seeds is None else seeds[b0:b1]),
+                                   _lib.ptr(None if anchors is None else anchors[b0:b1])) + args[4:]
+                self._check(self.L.ts_pixelcnn_sample_clips(*args, C.byref(c), clip[b0:b1].ctypes.data, self._s()),
+                            "ts_pixelcnn_sample_clips")
+            elif style is not None:
                 c = _ctl_struct(temperature, top_k, top_p, min_p, pz, kz) if ctl else None
                 args = args[:3] + (_lib.ptr(style[b0:b1]), self.pixelcnn_ncls, _lib.ptr(nz),
                                    _lib.ptr(None if seeds is None else seeds[b0:b1]),
@@ -570,8 +672,14 @@ class Engine:
         (ts_body_sample_seeded), as in ``pixelcnn_generate``.  ``anchors`` [B,T,2] pins draws as in ``pixelcnn_generate``
         (ts_body_sample_anchored; one synchronisation for a device tensor); the poses decode the resulting codes.
         ``style`` [B,T,ncls] or [B,ncls]: a speaker schedule as in ``pixelcnn_generate`` (ts_body_sample_styled; label
-        may then be None)."""
-        ctl = _controlled(temperature, top_k, noise, want_logp, top_p, min_p, want_kept, seeds)
+        may then be None).  Per-clip ``temperature`` / ``top_k`` / ``top_p`` / ``min_p`` as in ``pixelcnn_generate``
+        (ts_body_sample_clips); each clip's poses decode its own codes."""
+        clip = None
+        if per_clip(temperature, top_k, top_p, min_p):
+            clip = check_clip_controls(temperature, top_k, top_p, min_p, mfcc.shape[0])
+            ctl = _clip_source(clip, noise, seeds)
+        else:
+            ctl = _controlled(temperature, top_k, noise, want_logp, top_p, min_p, want_kept, seeds)
         mfcc = self._dev(mfcc, torch.float32)
         if label is None and style is None:
             raise ValueError("body_generate: label is required without style")
@@ -594,7 +702,14 @@ class Engine:
             nz = noise if (full or noise is None) else noise[:, b0:b1].contiguous()
             args = (self.h, _lib.ptr(mfcc[b0:b1]), _lib.ptr(None if label is None else label[b0:b1]), _lib.ptr(nz),
                     _lib.ptr(None if codes is None else codes[b0:b1]), _lib.ptr(poses[b0:b1]), b1 - b0, M)
-            if style is not None:
+            if clip is not None:
+                c = _ctl_struct(1.0, 0, 1.0, 0.0, None if logp is None else logp[b0:b1], None if kept is None else kept[b0:b1])
+                args = args[:3] + (_lib.ptr(None if style is None else style[b0:b1]), self.pixelcnn_ncls, _lib.ptr(nz),
+                                   _lib.ptr(None if seeds is None else seeds[b0:b1]),
+                                   _lib.ptr(None if anchors is None else anchors[b0:b1])) + args[4:]
+                self._check(self.L.ts_body_sample_clips(*args, C.byref(c), clip[b0:b1].ctypes.data, self._s()),
+                            "ts_body_sample_clips")
+            elif style is not None:
                 c = None
                 if ctl:
                     c = _ctl_struct(temperature, top_k, top_p, min_p, None if logp is None else logp[b0:b1],

@@ -10,7 +10,7 @@ import torch
 
 from ..data_utils.lower_body import c_index_3d, c_index_6d
 from ..data_utils.utils import get_mfcc_sepa, get_mfcc_ta, load_wav
-from ..engine import check_sample_controls, check_style, resolve_clip_seeds, sample_controls
+from ..engine import check_clip_controls, check_sample_controls, check_style, per_clip, resolve_clip_seeds, sample_controls, sampled
 from .base import draw_sampler_noise, resolve_device, shared_engine, strip_module
 
 
@@ -157,14 +157,18 @@ class TrainWrapper:
 
         ``style`` [B,T,4] per-row or [B,4] per-clip speaker weights (Engine.check_style: convex mixtures, float): the
         prior is conditioned on that mixture of its speaker embeddings instead of ``id``, which is then not read.  A
-        one-hot row of speaker s is exactly ``id = s``; a fade between two one-hot rows changes style over those rows."""
+        one-hot row of speaker s is exactly ``id = s``; a fade between two one-hot rows changes style over those rows.
+
+        Per-clip controls: ``temperature``, ``top_k``, ``top_p`` and ``min_p`` each take a scalar or one value per clip (a
+        length-B sequence, 1-D array or tensor; Engine.pixelcnn_generate), so one batch serves clips with different
+        settings; clip b draws what it draws alone under its own values.  Noise is drawn when any clip samples."""
         mfcc = aud.to(torch.float32)
         B, _, M = mfcc.shape
         T = self.engine.latent_rows(M)
         seeds = self._seeds(clip_seeds, B, noise_fn)
         noise = self._draw_noise(T, B, noise_fn, temperature, top_k, top_p, min_p, seeds)
         ctl = sample_controls(temperature, top_k, keep_logp, top_p, min_p)
-        if noise is None and seeds is not None and float(temperature) > 0:
+        if noise is None and seeds is not None and sampled(temperature):
             ctl["seeds"] = seeds
         if anchors is not None:
             ctl["anchors"] = anchors
@@ -177,10 +181,13 @@ class TrainWrapper:
         return poses
 
     def _draw_noise(self, T, B, noise_fn, temperature, top_k, top_p=1.0, min_p=0.0, seeds=None):
-        """[2T,B,2048] Exp(1) draws (RNG contract), or None for greedy decoding and seeded sampling (controls validated
-        first)."""
-        check_sample_controls(temperature, top_k, top_p, min_p)
-        if float(temperature) == 0 or seeds is not None:
+        """[2T,B,2048] Exp(1) draws (RNG contract), or None for greedy decoding (every clip greedy) and seeded sampling
+        (controls validated first, per clip when given per clip)."""
+        if per_clip(temperature, top_k, top_p, min_p):
+            check_clip_controls(temperature, top_k, top_p, min_p, B)
+        else:
+            check_sample_controls(temperature, top_k, top_p, min_p)
+        if not sampled(temperature) or seeds is not None:
             return None
         return self._noise(T, B) if noise_fn is None else noise_fn(T, B)
 
@@ -202,14 +209,15 @@ class TrainWrapper:
         ``clip_seeds`` as in ``generate``; with ``pre_latents`` the chunk's draws are keyed by their absolute rows (after
         the T0 rows of the previous chunk), so a seeded clip's noise does not depend on where it is cut into chunks.
         ``anchors`` [B,T,2] cover this chunk's T rows (as in ``generate``); with ``pre_latents`` they pin rows after the
-        prefix.  ``style`` [B,T0+T,4] (or [B,4]) as in ``generate``, its rows covering the prefix and the chunk."""
+        prefix.  ``style`` [B,T0+T,4] (or [B,4]) as in ``generate``, its rows covering the prefix and the chunk.  Per-clip
+        controls as in ``generate``."""
         a = self.engine.audio_encode(aud_feat.transpose(1, 2).contiguous())            # [B,256,T]
         T = a.shape[2]
         label = id.reshape(-1)
         seeds = self._seeds(clip_seeds, B, noise_fn)
         noise = self._draw_noise(T, B, noise_fn, temperature, top_k, top_p, min_p, seeds)
         ctl = sample_controls(temperature, top_k, keep_logp, top_p, min_p)
-        if noise is None and seeds is not None and float(temperature) > 0:
+        if noise is None and seeds is not None and sampled(temperature):
             ctl["seeds"] = seeds
         if anchors is not None:
             ctl["anchors"] = anchors
@@ -232,7 +240,7 @@ class TrainWrapper:
         """continuity=True (:244-269): a 2 s prefix, then the rest conditioned on the prefix's latents and audio.  The two
         chunks go through the audio encoder separately and are DECODED separately, so each chunk sees zero padding at the
         2 s seam.  ``style`` covers the whole clip (rows T_a + T_b): chunk 0 gets rows [0, T_a), chunk 1, whose prefix is
-        chunk 0, all of them."""
+        chunk 0, all of them.  Per-clip controls apply to both chunks of their clip."""
         aud_feat, gap = get_mfcc_sepa(aud_fn, sr=sr, fps=fps)                 # (M0+M1, 64), M0
         feat = torch.from_numpy(np.ascontiguousarray(np.asarray(aud_feat, dtype=np.float32)))[None].repeat(B, 1, 1)   # [B,M,64]
         label = torch.tensor([0]) if id is None else id.reshape(-1).repeat(B)

@@ -10,7 +10,7 @@ from __future__ import annotations
 
 import torch
 
-from .engine import Engine, check_anchors, check_style, resolve_clip_seeds, sample_controls
+from .engine import Engine, check_anchors, check_clip_controls, check_style, per_clip, resolve_clip_seeds, sample_controls, sampled
 from .nets.base import draw_sampler_noise
 
 
@@ -91,7 +91,9 @@ class WholeBody:
         the codes a later call can anchor to.
         ``style`` [B,T,ncls] or [B,ncls]: a speaker schedule for the body prior (s2g_body_pixel.generate), ``label`` is then
         not read.  The face path keeps the demo's zero id (demo.py:173-181) whatever the style: the body prior is the only
-        net styled here (s2g_face.generate_ids takes a soft id for the face)."""
+        net styled here (s2g_face.generate_ids takes a soft id for the face).
+        ``temperature`` / ``top_k`` / ``top_p`` / ``min_p`` may each be given per clip (s2g_body_pixel.generate): one batch
+        serves clips with different settings, on the overlapped and the sequential path alike."""
         B, _, M = mfcc.shape
         frame = wave.shape[1] * 30 // 16000
         T = self.e.latent_rows(M)
@@ -100,9 +102,9 @@ class WholeBody:
         if noise is not None and clip_seeds is not None:
             raise ValueError("WholeBody.generate: noise and clip_seeds are two noise sources; give one")
         seeds = resolve_clip_seeds(clip_seeds, B)
-        if seeds is not None and float(temperature) > 0:
+        if seeds is not None and sampled(temperature):
             ctl["seeds"] = seeds
-        elif noise is None and float(temperature) > 0:
+        elif noise is None and sampled(temperature):
             noise = draw_sampler_noise(T, B, self.device, per_step=per_step_noise)
         if anchors is not None:
             ctl["anchors"] = anchors
@@ -189,7 +191,8 @@ class WholeBody:
         its meaning (the torch stream of the full-batch noise) and is not used with ``clip_seeds``.
         ``anchors`` [B,T,2] (as in ``generate``, for the full batch): rank r passes the rows of its shard, so the gathered
         result equals ``generate`` with the same anchors on one GPU.  ``style`` [B,T,ncls] or [B,ncls] (full batch, as in
-        ``generate``): rank r passes its shard's rows."""
+        ``generate``): rank r passes its shard's rows.  Per-clip ``temperature`` / ``top_k`` / ``top_p`` / ``min_p`` (full
+        batch, as in ``generate``): rank r passes its shard's values."""
         B, _, M = mfcc.shape
         lo, hi = shard_range(B, rank, world)
         T = self.e.latent_rows(M)
@@ -198,6 +201,9 @@ class WholeBody:
         ctl = dict(temperature=temperature, top_k=top_k, keep_logp=keep_logp) if sc else {}
         if "top_p" in sc:
             ctl.update(top_p=top_p, min_p=min_p)
+        if per_clip(temperature, top_k, top_p, min_p):
+            cc = check_clip_controls(temperature, top_k, top_p, min_p, B)[lo:hi]
+            ctl.update(temperature=cc["temperature"], top_k=cc["top_k"], top_p=cc["top_p"], min_p=cc["min_p"])
         if noise_full is not None and clip_seeds is not None:
             raise ValueError("WholeBody.generate_sharded: noise_full and clip_seeds are two noise sources; give one")
         seeds = resolve_clip_seeds(clip_seeds, B)
@@ -207,7 +213,7 @@ class WholeBody:
             ctl["style"] = check_style(style, B, T, self.e.pixelcnn_ncls)[lo:hi]
         if seeds is not None:
             ctl["clip_seeds"] = seeds[lo:hi]
-        elif noise_full is None and float(temperature) > 0:
+        elif noise_full is None and sampled(temperature):
             g = None
             if seed is not None:
                 g = torch.Generator(device=self.device)
