@@ -227,6 +227,36 @@ int ts_pixelcnn_sample_clips(ts_engine* e, const float* aud, const int64_t* labe
                              const float* noise, const int64_t* seeds, const int64_t* anchors, int64_t* idx_out,
                              float* logits_out, int B, int T, const int64_t* pre_latents, int T0, const ts_sample_ctl* ctl,
                              const ts_clip_ctl* clip_ctl, void* stream);
+/* ---- logit shaping: a repetition penalty over each clip's recent codes and an additive per-code bias ----------------
+ * One entry per clip (clip_shape, HOST memory): */
+typedef struct ts_clip_shape {
+  float repetition_penalty;   /* theta: finite, >= 1; 1 = off */
+  int32_t repetition_window;  /* W >= 1 latent rows */
+} ts_clip_shape;
+/* ts_pixelcnn_sample_clips where the raw logits l of every sampled draw are shaped before the controls act.
+ * code_bias [B,2,2048] (DEVICE, may be NULL): one row per clip and column (0 = body codebook, 1 = hand codebook); each value
+ * finite with |v| <= 1e4, or -inf, and each row with at least one finite value (the kernel survives any data: a row of
+ * -inf draws code 0, the first-index argmax).  For the draw at absolute latent row r (pre_latents rows included), column
+ * c, of clip b:
+ *  1. Penalty.  H = the codes at column c in rows max(0, r - W) .. r - 1 of clip b: pre_latents rows and pinned draws
+ *     included, column 1 of row r not seen by column 0 nor the other way.  Every code n in H (once, however often it
+ *     occurs) gets l_n = l_n > 0 ? l_n / theta : l_n * theta, IEEE fp32, no contraction.
+ *  2. Bias.  l_n = l_n + bias[b][c][n] (fp32 add, round to nearest).
+ *  3. The controls of ts_pixelcnn_sample_clips (temperature, top_k, top_p, min_p, the argmax(p / q) draw, greedy as the
+ *     first-index argmax, the overflow fallback) act on the shaped logits.
+ *  4. A code whose shaped logit is -inf is never drawn and is not counted in kept_out.
+ *  5. logp_out is still the log-probability under the raw (untempered, unshaped) prior, as in every sampling call.
+ *  6. A pinned draw (anchors) is not shaped: its log p and kept_out = 0 are unchanged; its code enters later histories.
+ * clip_shape [B] (HOST, may be NULL = theta 1 for every clip) is checked on the host (TS_ERR_INVALID, the message names
+ * the clip) and copied to engine-owned device memory on `stream` with no synchronisation.  theta = 1 and no bias: the
+ * clip draws what ts_pixelcnn_sample_clips draws, bit for bit.  clip_ctl = NULL: ctl's scalar controls (or the default
+ * draw when ctl is NULL too).  Both clip_shape and code_bias NULL: the call equals ts_pixelcnn_sample_clips with the same
+ * arguments, bit for bit and with its launches; otherwise it runs that call's kernels (one extra host-to-device copy). */
+int ts_pixelcnn_sample_shaped(ts_engine* e, const float* aud, const int64_t* label, const float* style, int ncls,
+                              const float* noise, const int64_t* seeds, const int64_t* anchors, int64_t* idx_out,
+                              float* logits_out, int B, int T, const int64_t* pre_latents, int T0, const ts_sample_ctl* ctl,
+                              const ts_clip_ctl* clip_ctl, const ts_clip_shape* clip_shape, const float* code_bias,
+                              void* stream);
 /* GatedPixelCNN.forward (teacher forced), :130-150, for rows [0,T): logits_out [B,2048,T,2]. */
 int ts_pixelcnn_logits(ts_engine* e, const float* aud, const int64_t* label, const int64_t* codes,
                        float* logits_out, int B, int T, void* stream);
@@ -323,6 +353,12 @@ int ts_body_sample_styled(ts_engine* e, const float* mfcc, const int64_t* label,
 int ts_body_sample_clips(ts_engine* e, const float* mfcc, const int64_t* label, const float* style, int ncls,
                          const float* noise, const int64_t* seeds, const int64_t* anchors, int64_t* codes, float* poses,
                          int B, int M, const ts_sample_ctl* ctl, const ts_clip_ctl* clip_ctl, void* stream);
+/* ts_body_sample_clips with the logit shaping of ts_pixelcnn_sample_shaped (clip_shape [B] in host memory, code_bias
+ * [B,2,2048] on the device); the poses decode each clip's codes.  Both NULL equals ts_body_sample_clips. */
+int ts_body_sample_shaped(ts_engine* e, const float* mfcc, const int64_t* label, const float* style, int ncls,
+                          const float* noise, const int64_t* seeds, const int64_t* anchors, int64_t* codes, float* poses,
+                          int B, int M, const ts_sample_ctl* ctl, const ts_clip_ctl* clip_ctl,
+                          const ts_clip_shape* clip_shape, const float* code_bias, void* stream);
 
 /* Audio front-end of get_mfcc_ta, data_utils/utils.py:148-177 (SURVEY.md §8f-1): wave [B,N] mono at
  * `sr` Hz -> torchaudio Resample(sr, 22000) -> MFCC(64 coefficients, n_fft 2048, hop 734 = 30 fps, 256 HTK

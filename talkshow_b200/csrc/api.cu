@@ -242,11 +242,12 @@ extern "C" int ts_vq_dim(ts_engine* e, int which) {
 // ctl = nullptr: the default sampler (ts_body_generate); else the sampling controls of ts_body_sample.
 // seeds (ts_body_sample_seeded): per-clip seeds in place of noise.  anchors (ts_body_sample_anchored): pinned draws.
 // style (ts_body_sample_styled): per-row speaker weights in place of label.  clip_ctl (ts_body_sample_clips): per-clip
-// controls (host, validated) in place of ctl's four.
+// controls (host, validated) in place of ctl's four.  clip_shape / code_bias (ts_body_sample_shaped): logit shaping.
 static void body_generate(ts_engine* e, const float* mfcc, const int64_t* label, const float* noise, int64_t* codes,
                           float* poses, int B, int M, void* stream, const SampleCtl* ctl, const int64_t* seeds = nullptr,
                           const int64_t* anchors = nullptr, const float* style = nullptr,
-                          const ts_clip_ctl* clip_ctl = nullptr) {
+                          const ts_clip_ctl* clip_ctl = nullptr, const ts_clip_shape* clip_shape = nullptr,
+                          const float* code_bias = nullptr) {
   ts::require_device(e);
   if (!e->conv || !e->conv->audio_loaded) fail(TS_ERR_NOT_LOADED, "audio encoder weights not loaded");
   if (!e->conv->vq[0].loaded || !e->conv->vq[1].loaded) fail(TS_ERR_NOT_LOADED, "vq weights not loaded");
@@ -263,7 +264,8 @@ static void body_generate(ts_engine* e, const float* mfcc, const int64_t* label,
     Act3 a = run_trunk(e, e->conv->audio, x, s);          // [B,T,256] channel-last, pad 1
     int64_t* idx = e->ws.alloc<int64_t>((size_t)B * T * 2);
     int64_t* idx_c = e->ws.alloc<int64_t>((size_t)B * T * 2);  // [2][B][T] column-split copy
-    pixelcnn_generate_act(e, a, label, noise, idx, nullptr, B, T, nullptr, 0, s, false, ctl, seeds, anchors, style, clip_ctl);
+    pixelcnn_generate_act(e, a, label, noise, idx, nullptr, B, T, nullptr, 0, s, false, ctl, seeds, anchors, style, clip_ctl,
+                          clip_shape, code_bias);
     split_codes(e, idx, idx_c, B, T, codes, s);
     const int c0 = e->conv->vq[0].out_dim, c1 = e->conv->vq[1].out_dim;   // 39 + 90 (axis-angle) or 78 + 180 (6-D)
     // Small batches: each decoder is a chain of ~20 launches that fill a few SMs, so the hand decoder runs on a second
@@ -383,5 +385,22 @@ extern "C" int ts_body_sample_clips(ts_engine* e, const float* mfcc, const int64
   SampleCtl c;   // logp_out / kept_out of ctl; the draws' controls come from clip_ctl
   if (ctl) { c.logp_out = ctl->logp_out; c.kept_out = ctl->kept_out; }
   body_generate(e, mfcc, label, noise, codes, poses, B, M, stream, &c, seeds, anchors, style, clip_ctl);
+  TS_API_END(e)
+}
+
+extern "C" int ts_body_sample_shaped(ts_engine* e, const float* mfcc, const int64_t* label, const float* style, int ncls,
+                                     const float* noise, const int64_t* seeds, const int64_t* anchors, int64_t* codes,
+                                     float* poses, int B, int M, const ts_sample_ctl* ctl, const ts_clip_ctl* clip_ctl,
+                                     const ts_clip_shape* clip_shape, const float* code_bias, void* stream) {
+  if (!clip_shape && !code_bias)
+    return ts_body_sample_clips(e, mfcc, label, style, ncls, noise, seeds, anchors, codes, poses, B, M, ctl, clip_ctl, stream);
+  TS_API_BEGIN(e)
+  ts::require_device(e);
+  if (!e->pix) fail(TS_ERR_NOT_LOADED, "pixelcnn weights not loaded");
+  if (B <= 0) fail(TS_ERR_INVALID, "ts_body_sample_shaped: B=%d", B);
+  check_style(e, label, style, ncls, "ts_body_sample_shaped");
+  if (clip_shape) check_clip_shape(clip_shape, B, "ts_body_sample_shaped");
+  const SampleCtl c = shaped_ctl(ctl, clip_ctl, B, noise, seeds, "ts_body_sample_shaped");
+  body_generate(e, mfcc, label, noise, codes, poses, B, M, stream, &c, seeds, anchors, style, clip_ctl, clip_shape, code_bias);
   TS_API_END(e)
 }

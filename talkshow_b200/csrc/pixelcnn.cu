@@ -484,6 +484,10 @@ struct PixArgs {
   // per-clip controls (ts_pixelcnn_sample_clips), read by the WARP instantiations only: [B] (device), indexed by the
   // global clip index; or null (the scalar controls above)
   const ts_clip_ctl* clip_ctl;
+  // logit shaping (ts_pixelcnn_sample_shaped), read by the WARP instantiations only, by global clip index: [B] (device)
+  // repetition penalty and window, or null (theta 1); [B][2][2048] (device) code bias, or null
+  const ts_clip_shape* clip_shape;
+  const float* code_bias;
 };
 
 // The sampling controls of clip m (global index): its entry of A.clip_ctl, else the call's scalar controls.  Every draw
@@ -506,6 +510,71 @@ __device__ __forceinline__ DrawCtl draw_ctl(const Args& A, int m) {
 template <class Args>
 __device__ __forceinline__ float draw_temperature(const Args& A, int m) {
   return A.clip_ctl ? __ldg(&A.clip_ctl[m].temperature) : A.temperature;
+}
+
+// ---- logit shaping: the rule of ts_pixelcnn_sample_shaped (include/talkshow_b200.h) --------------------------------
+// The sample stage's scratch words (red) past draw_controlled's 578 that the shaping stages into: the history bitmap of
+// the draw (64 words, one bit per code) and the clip's bias row of the draw's column (2048 floats, each read back by the
+// thread that wrote it).
+constexpr int SHAPE_BITS = 1024, SHAPE_BIAS = 2048, SHAPE_END = SHAPE_BIAS + PIX_NCODE;
+static_assert(sizeof(ts_clip_shape) == 8, "ts_clip_shape is read as one 8-byte load");
+struct ShapeCtl {
+  float theta;
+  int window;
+};
+template <class Args>
+__device__ __forceinline__ ShapeCtl shape_ctl(const Args& A, int m) {
+  if (!A.clip_shape) return {1.f, 0};
+  const int2 v = __ldg(reinterpret_cast<const int2*>(A.clip_shape) + m);
+  return {__int_as_float(v.x), v.y};
+}
+
+// Stages what the shaping of draw (r, c) of clip m reads: the bitmap of the codes at column c in rows max(0, r - W) ..
+// r - 1 (rows < T0 from pre, later rows from this call's idx_out, written earlier in the launch by the CTA that samples
+// clip m: coherent L2 loads, never the read-only path) and the bias row.  Everything it reads is final before the sample
+// stage starts, so both persistent executors stage it before their barrier wait, where it overlaps the wait; the bitmap is
+// published by the caller's next barrier.  Out-of-range history codes are skipped.  Uniform over the CTA (one clip).
+template <class Args, class Bar>
+__device__ __forceinline__ void shape_stage(const Args& A, int m, int r, int c, float* red, Bar bar) {
+  const int tid = threadIdx.x;
+  const ShapeCtl sc = shape_ctl(A, m);
+  if (sc.theta != 1.f) {
+    unsigned* bits = reinterpret_cast<unsigned*>(red + SHAPE_BITS);
+    if (tid < PIX_NCODE / 32) bits[tid] = 0u;
+    bar();
+    const int lo = sc.window >= r ? 0 : r - max(sc.window, 0);
+    for (int i = lo + tid; i < r; i += 256) {
+      const int64_t* src = i < A.T0 ? A.pre + ((size_t)m * A.T0 + i) * 2 + c
+                                    : A.idx_out + ((size_t)m * (A.Ttot - A.T0) + (i - A.T0)) * 2 + c;
+      const long long code = __ldcg(reinterpret_cast<const long long*>(src));
+      if (code >= 0 && code < PIX_NCODE) atomicOr(&bits[code >> 5], 1u << (code & 31));
+    }
+  }
+  if (A.code_bias) {
+    const float* b = A.code_bias + ((size_t)m * 2 + c) * PIX_NCODE;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) red[SHAPE_BIAS + tid + 256 * j] = __ldg(b + tid + 256 * j);
+  }
+}
+
+// Shapes the raw logits l of clip m's draw in place from what shape_stage staged: the penalty on the history's codes,
+// then the bias.  Returns whether the draw is shaped (theta != 1 or a bias), the same in every thread.
+template <class Args>
+__device__ __forceinline__ bool shape_logits(const Args& A, int m, const float* red, float (&l)[8]) {
+  const int tid = threadIdx.x;
+  const ShapeCtl sc = shape_ctl(A, m);
+  if (sc.theta != 1.f) {
+    const unsigned* bits = reinterpret_cast<const unsigned*>(red + SHAPE_BITS);
+#pragma unroll
+    for (int j = 0; j < 8; ++j)   // code tid + 256 j: word (tid >> 5) + 8 j, bit tid & 31
+      if ((bits[(tid >> 5) + 8 * j] >> (tid & 31)) & 1u)
+        l[j] = l[j] > 0.f ? __fdiv_rn(l[j], sc.theta) : __fmul_rn(l[j], sc.theta);
+  }
+  if (A.code_bias) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) l[j] = __fadd_rn(l[j], red[SHAPE_BIAS + tid + 256 * j]);
+  }
+  return sc.theta != 1.f || A.code_bias != nullptr;
 }
 
 // The speaker weights of row r of clip m (global index) under A.style, or null for a padding sample (m >= B).
@@ -1237,7 +1306,8 @@ __device__ __forceinline__ void draw_logp(const float (&l)[8], float mx, long lo
 //   argmax((exp(s - max s) / sum) / q) with first-index ties, over the kept codes only.
 //   top_p < 1 / min_p > 0 (ts_pixelcnn_sample_ctl) drop further codes before the sum: with e = exp(s - max s) of the
 //   codes top-k kept and the integer mass w = rint(e 2^32), top-p keeps the codes at or above nucleus_key, min-p those
-//   with e >= min_p.  kept_dst (may be null) receives the size of the final keep set (1 for a greedy draw).
+//   with e >= min_p.  kept_dst (may be null) receives the size of the final keep set (1 for a greedy draw).  A code whose
+//   logit is -inf (a shaped draw's ban, ts_pixelcnn_sample_shaped) is never in the keep set.
 // At temperature 1 without truncation this is the default sampler's arithmetic step for step (s == l).
 // A temperature so small that max(l) / temperature overflows makes every p / q NaN, so no code wins the draw: the code is
 // then the greedy one, the limit of the tempered draw as the temperature goes to 0.  The returned code always lies in
@@ -1263,7 +1333,7 @@ __device__ __forceinline__ long long draw_controlled(const float (&l)[8], const 
   const bool truncate = !greedy && ((top_k > 0 && top_k < PIX_NCODE) || nucleus || floor_p);
   bool keep[8];
 #pragma unroll
-  for (int j = 0; j < 8; ++j) keep[j] = true;
+  for (int j = 0; j < 8; ++j) keep[j] = l[j] != -INFINITY;
   uint32_t key[8];
   if (!greedy && ((top_k > 0 && top_k < PIX_NCODE) || nucleus)) {
 #pragma unroll
@@ -1272,7 +1342,7 @@ __device__ __forceinline__ long long draw_controlled(const float (&l)[8], const 
   if (!greedy && top_k > 0 && top_k < PIX_NCODE) {
     const uint32_t kth = kth_largest_key(key, top_k, hist, sel, bar);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) keep[j] = key[j] >= kth;
+    for (int j = 0; j < 8; ++j) keep[j] = keep[j] && key[j] >= kth;
   }
   float sum_raw = 0.f;
   long long code;
@@ -1439,8 +1509,15 @@ __device__ void run_sample_task(const PixTask& t, const PixArgs& A, int r, int m
             draw_noise(A, r, c, m, qv);
           }
         }
-        code = draw_controlled(l, qv, dc.temperature, dc.top_k, dc.top_p, dc.min_p, red, A.logp_out ? A.logp_out + at : nullptr,
+        const bool shaped = shape_logits(A, m, red, l);
+        float* logp = A.logp_out ? A.logp_out + at : nullptr;
+        code = draw_controlled(l, qv, dc.temperature, dc.top_k, dc.top_p, dc.min_p, red, shaped ? nullptr : logp,
                                A.kept_out ? A.kept_out + at : nullptr, CtaBar());
+        if (shaped && logp) {   // log p under the raw prior: the LOG slot still holds the unshaped logits
+#pragma unroll
+          for (int j = 0; j < 8; ++j) l[j] = __ldcg(A.arena + A.lay.LOG + ax<MB>(tid + 256 * j, m));
+          draw_pinned(l, code, red, logp, nullptr, CtaBar());
+        }
       }
     } else {
       code = A.pre[((size_t)m * A.T0 + r) * 2 + c];
@@ -1523,6 +1600,7 @@ __device__ void run_sample_task(const PixTask& t, const PixArgs& A, int r, int m
 }
 
 constexpr int PIX_MAXSTAGES = 160;  // this CTA's column of the stage table is kept in shared memory
+static_assert(SHAPE_END <= 8 * PIX_MAXROWS * 64, "the shaping inputs are staged in the sampler's scratch");
 constexpr size_t PIX_SMEM = (size_t)(2 * PIX_WBUF + 8 * PIX_MAXROWS * 64) * sizeof(float) + 64 + PIX_MAXSTAGES * sizeof(PixTask);
 
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
@@ -1548,7 +1626,18 @@ __global__ void __launch_bounds__(PIX_THREADS, 1) pixelcnn_kernel(PixArgs A, int
     // debug cross-check mode: one launch per stage, weights copied synchronously
     const PixTask t = A.table[(size_t)s_single * A.ncta + cta];
     if (!task_active(t, r_single, A.log_r0)) return;
-    if (t.epi == EPI_SAMPLE) { if (cta < A.B) run_sample_task<MB, false, WARP>(t, A, r_single, cta, red); return; }
+    if (t.epi == EPI_SAMPLE) {
+      if (cta < A.B) {
+        if constexpr (WARP) {   // the shaping inputs of the draw (ts_pixelcnn_sample_shaped)
+          if (r_single >= A.T0 && (A.clip_shape || A.code_bias)) {
+            shape_stage(A, cta, r_single, t.col, red, CtaBar());
+            __syncthreads();
+          }
+        }
+        run_sample_task<MB, false, WARP>(t, A, r_single, cta, red);
+      }
+      return;
+    }
     const int nf = (t.K + 1) * t.rpad;
     for (int i = tid; i < nf; i += PIX_THREADS) wbuf[i] = A.blob[t.wofs + i];
     __syncthreads();
@@ -1601,6 +1690,10 @@ __global__ void __launch_bounds__(PIX_THREADS, 1) pixelcnn_kernel(PixArgs A, int
     float qpre[8];
     if (active && t.epi == EPI_SAMPLE && cta < A.B && r >= A.T0 && (!WARP || draw_temperature(A, cta) > 0.f))   // greedy: no noise
       draw_noise(A, r, t.col, cta, qpre);
+    if constexpr (WARP) {   // the shaping inputs of this draw (ts_pixelcnn_sample_shaped), likewise before the wait
+      if (active && t.epi == EPI_SAMPLE && cta < A.B && r >= A.T0 && (A.clip_shape || A.code_bias))
+        shape_stage(A, cta, r, t.col, red, CtaBar());
+    }
     if (has_w) { mbar_wait(&bars[buf], uses[buf] & 1u); uses[buf]++; }
     unsigned long long* tr = nullptr;
     if constexpr (TRACE) {
@@ -1669,7 +1762,8 @@ __global__ void logits_to_ref_kernel(const float* __restrict__ in, float* __rest
 static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t* label, const float* noise, int noise_B,
                            int64_t* idx_out, float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s,
                            bool logits_all, const SampleCtl* ctl, const int64_t* seeds, const int64_t* anchors,
-                           const float* style, const ts_clip_ctl* clip_ctl) {
+                           const float* style, const ts_clip_ctl* clip_ctl, const ts_clip_shape* clip_shape,
+                           const float* code_bias) {
   PixelPlan* P = e->pix;
   Plan3* Q = (Plan3*)P->p3;
   const int Ttot = T0 + T, D = P->D;
@@ -1697,7 +1791,7 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
 
   if (v3) {   // cluster-resident executor (pixelcnn3.inc): any batch size, clusters of 16 CTAs per 4 / 8 samples
     launch_pixelcnn3(e, P, Q, audv, audh, label, noise, idx_out, logits_out, B, T0, Ttot, pre, logits_all, arena3, MB3, s, ctl, seeds,
-                     anchors, style, clip_ctl);
+                     anchors, style, clip_ctl, clip_shape, code_bias);
     return;
   }
   if (B > PIX_MB)
@@ -1732,6 +1826,7 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
   A.anchors = anchors;
   A.style = style; A.cls_w = P->d_cls; A.ncls = P->nclasses;
   A.clip_ctl = clip_ctl;
+  A.clip_shape = clip_shape; A.code_bias = code_bias;
   if (e->pixel_mode == 0) {
     // A/B switch: 0 = burst loads + scalar FFMA, 4 = pipelined loads + scalar FFMA, 5 (default) = pipelined loads + paired FMAs (fma2)
     static const int pipe = getenv("TS_PIX_PIPE") ? atoi(getenv("TS_PIX_PIPE")) : 5;
@@ -1806,18 +1901,22 @@ void pixel_destroy(ts_engine* e) {
 void pixelcnn_generate_act(ts_engine* e, const Act3& aud, const int64_t* label, const float* noise, int64_t* idx_out,
                            float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s, bool logits_all,
                            const SampleCtl* ctl, const int64_t* seeds, const int64_t* anchors, const float* style,
-                           const ts_clip_ctl* clip_ctl) {
+                           const ts_clip_ctl* clip_ctl, const ts_clip_shape* clip_shape, const float* code_bias) {
   if (!e->pix) fail(TS_ERR_NOT_LOADED, "pixelcnn weights not loaded");
-  // an anchored, styled or per-clip call always runs the WARP kernels; without controls at temperature 1, top_k 0 (the
-  // default draw's bits)
+  // an anchored, styled, per-clip or shaped call always runs the WARP kernels; without controls at temperature 1, top_k 0
+  // (the default draw's bits)
   const SampleCtl dflt;
-  if ((anchors || style || clip_ctl) && !ctl) ctl = &dflt;
-  // per-clip controls: host entries (validated by the caller) -> workspace, in stream order before the sampler reads them
+  if ((anchors || style || clip_ctl || clip_shape || code_bias) && !ctl) ctl = &dflt;
+  // per-clip controls and shaping: host entries (validated by the caller) -> workspace, in stream order before the
+  // sampler reads them
   ts_clip_ctl* dclip = clip_ctl ? e->ws.alloc<ts_clip_ctl>((size_t)B) : nullptr;
   if (dclip && !e->ws.sizing)
     TS_CUDA(cudaMemcpyAsync(dclip, clip_ctl, (size_t)B * sizeof(ts_clip_ctl), cudaMemcpyHostToDevice, s));
+  ts_clip_shape* dshape = clip_shape ? e->ws.alloc<ts_clip_shape>((size_t)B) : nullptr;
+  if (dshape && !e->ws.sizing)
+    TS_CUDA(cudaMemcpyAsync(dshape, clip_shape, (size_t)B * sizeof(ts_clip_shape), cudaMemcpyHostToDevice, s));
   generate_chunk(e, aud, 0, label, noise, B, idx_out, logits_out, B, T, pre, T0, s, logits_all, ctl, seeds, anchors, style,
-                 dclip);
+                 dclip, dshape, code_bias);
 }
 
 void check_style(const ts_engine* e, const int64_t* label, const float* style, int ncls, const char* who) {
@@ -1862,6 +1961,30 @@ void check_clip_ctl(const ts_clip_ctl* clip_ctl, int B, const float* noise, cons
   if (sampled && (noise != nullptr) == (seeds != nullptr))
     fail(TS_ERR_INVALID, "%s: noise=%p seeds=%p (give exactly one; only a batch of greedy clips runs without)", who,
          (const void*)noise, (const void*)seeds);
+}
+
+SampleCtl shaped_ctl(const ts_sample_ctl* ctl, const ts_clip_ctl* clip_ctl, int B, const float* noise, const int64_t* seeds,
+                     const char* who) {
+  SampleCtl c;
+  if (clip_ctl) {   // logp_out / kept_out of ctl; the draws' controls come from clip_ctl
+    check_clip_ctl(clip_ctl, B, noise, seeds, who);
+    if (ctl) { c.logp_out = ctl->logp_out; c.kept_out = ctl->kept_out; }
+    return c;
+  }
+  if (ctl) c = sample_ctl_of(ctl);
+  check_sample_ctl(c, noise, seeds);
+  check_anchored_source(&c, noise, seeds, who);
+  return c;
+}
+
+void check_clip_shape(const ts_clip_shape* clip_shape, int B, const char* who) {
+  for (int b = 0; b < B; ++b) {
+    const ts_clip_shape& c = clip_shape[b];
+    if (!std::isfinite(c.repetition_penalty) || !(c.repetition_penalty >= 1.f))
+      fail(TS_ERR_INVALID, "%s: clip %d: repetition_penalty %g (must be finite and >= 1)", who, b, (double)c.repetition_penalty);
+    if (c.repetition_window < 1)
+      fail(TS_ERR_INVALID, "%s: clip %d: repetition_window %d (must be >= 1)", who, b, c.repetition_window);
+  }
 }
 
 SampleCtl sample_ctl_of(const ts_sample_ctl* c) {
@@ -2004,7 +2127,8 @@ static void check_pix(ts_engine* e, int B, int T) {
 static void pixelcnn_generate_call(ts_engine* e, const float* aud, const int64_t* label, const float* noise, int64_t* idx_out,
                                    float* logits_out, int B, int T, const int64_t* pre_latents, int T0, void* stream,
                                    const SampleCtl* ctl, const int64_t* seeds = nullptr, const int64_t* anchors = nullptr,
-                                   const float* style = nullptr, const ts_clip_ctl* clip_ctl = nullptr) {
+                                   const float* style = nullptr, const ts_clip_ctl* clip_ctl = nullptr,
+                                   const ts_clip_shape* clip_shape = nullptr, const float* code_bias = nullptr) {
   check_pix(e, B, T);
   if (T0 < 0 || (T0 > 0 && !pre_latents)) fail(TS_ERR_INVALID, "pixelcnn: T0=%d without pre_latents", T0);
   if (ctl && !clip_ctl) check_sample_ctl(*ctl, noise, seeds);
@@ -2013,7 +2137,7 @@ static void pixelcnn_generate_call(ts_engine* e, const float* aud, const int64_t
     Act3 a = new_act(e, B, T0 + T, 256, 0, s);
     nct_to_act(e, aud, 256, a, s);
     pixelcnn_generate_act(e, a, label, noise, idx_out, logits_out, B, T, pre_latents, T0, s, false, ctl, seeds, anchors, style,
-                          clip_ctl);
+                          clip_ctl, clip_shape, code_bias);
   };
   e->ws.begin_sizing(); body();
   size_t need = e->ws.need;
@@ -2132,6 +2256,27 @@ extern "C" int ts_pixelcnn_sample_clips(ts_engine* e, const float* aud, const in
   if (ctl) { c.logp_out = ctl->logp_out; c.kept_out = ctl->kept_out; }
   pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, &c, seeds, anchors, style,
                          clip_ctl);
+  TS_API_END(e)
+}
+
+// clip_shape [B] (host): each clip's repetition penalty and window, validated here and copied to the workspace on the
+// call's stream; code_bias [B,2,2048] (device).  clip_ctl NULL: ctl's scalar controls.  Both NULL: ts_pixelcnn_sample_clips
+// with its launches and bits.
+extern "C" int ts_pixelcnn_sample_shaped(ts_engine* e, const float* aud, const int64_t* label, const float* style, int ncls,
+                                         const float* noise, const int64_t* seeds, const int64_t* anchors, int64_t* idx_out,
+                                         float* logits_out, int B, int T, const int64_t* pre_latents, int T0,
+                                         const ts_sample_ctl* ctl, const ts_clip_ctl* clip_ctl, const ts_clip_shape* clip_shape,
+                                         const float* code_bias, void* stream) {
+  if (!clip_shape && !code_bias)
+    return ts_pixelcnn_sample_clips(e, aud, label, style, ncls, noise, seeds, anchors, idx_out, logits_out, B, T, pre_latents,
+                                    T0, ctl, clip_ctl, stream);
+  TS_API_BEGIN(e)
+  check_pix(e, B, T);
+  check_style(e, label, style, ncls, "ts_pixelcnn_sample_shaped");
+  if (clip_shape) check_clip_shape(clip_shape, B, "ts_pixelcnn_sample_shaped");
+  const SampleCtl c = shaped_ctl(ctl, clip_ctl, B, noise, seeds, "ts_pixelcnn_sample_shaped");
+  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, &c, seeds, anchors, style,
+                         clip_ctl, clip_shape, code_bias);
   TS_API_END(e)
 }
 

@@ -93,11 +93,14 @@ SampleCtl sample_ctl_of(const ts_sample_ctl* c);
 // controls when ctl is null.  style [B,T0+T,ncls] (device): the speaker schedule of ts_pixelcnn_sample_styled (label
 // unread), likewise on the WARP kernels.  clip_ctl [B] (HOST, validated with check_clip_ctl): the per-clip controls of
 // ts_pixelcnn_sample_clips, copied to the workspace on s; each clip draws with its entry in place of ctl's four controls.
+// clip_shape [B] (HOST, validated with check_clip_shape) and code_bias [B,2,2048] (device): the logit shaping of
+// ts_pixelcnn_sample_shaped, likewise on the WARP kernels (clip_shape copied to the workspace on s).
 void pixelcnn_generate_act(ts_engine* e, const Act3& aud, const int64_t* label, const float* noise, int64_t* idx_out,
                            float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s,
                            bool logits_all = false, const SampleCtl* ctl = nullptr, const int64_t* seeds = nullptr,
                            const int64_t* anchors = nullptr, const float* style = nullptr,
-                           const ts_clip_ctl* clip_ctl = nullptr);
+                           const ts_clip_ctl* clip_ctl = nullptr, const ts_clip_shape* clip_shape = nullptr,
+                           const float* code_bias = nullptr);
 // The class terms of gate channel q (tanh half) and D + q (sigmoid half) under one row's speaker weights w[0..ncls)
 // (ts_pixelcnn_sample_styled): acc = w0 E[0][ch], then acc + w_s E[s][ch] for s = 1 .. ncls-1, every product and sum
 // rounded to fp32 without contraction.  tab: one layer's class_cond_embedding [ncls][2D]; w null (a padding sample of the
@@ -125,6 +128,13 @@ void check_anchored_source(const SampleCtl* ctl, const float* noise, const int64
 // The per-clip controls of ts_pixelcnn_sample_clips (TS_ERR_INVALID, naming the clip): every entry by the rules of
 // check_sample_ctl, and exactly one of noise and seeds when any clip samples (temperature > 0).  clip_ctl: B host entries.
 void check_clip_ctl(const ts_clip_ctl* clip_ctl, int B, const float* noise, const int64_t* seeds, const char* who);
+// The per-clip shaping of ts_pixelcnn_sample_shaped (TS_ERR_INVALID, naming the clip): a finite repetition_penalty >= 1
+// and a repetition_window >= 1.  clip_shape: B host entries.
+void check_clip_shape(const ts_clip_shape* clip_shape, int B, const char* who);
+// The controls of a shaped call: with clip_ctl, check_clip_ctl and ctl's logp_out / kept_out; else ctl's controls (the
+// default draw when ctl is NULL), checked with check_sample_ctl and check_anchored_source.
+SampleCtl shaped_ctl(const ts_sample_ctl* ctl, const ts_clip_ctl* clip_ctl, int B, const float* noise, const int64_t* seeds,
+                     const char* who);
 // idx [B,T,2] -> idx_c [2][B][T]; optionally copies idx to codes_out
 void split_codes(ts_engine* e, const int64_t* idx, int64_t* idx_c, int B, int T, int64_t* codes_out, cudaStream_t s);
 void pixel_destroy(ts_engine* e);

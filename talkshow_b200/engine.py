@@ -119,6 +119,117 @@ def check_clip_controls(temperature, top_k, top_p=1.0, min_p=0.0, B=None):
     return out
 
 
+# one entry of the per-clip logit shaping (include/talkshow_b200.h ts_clip_shape)
+CLIP_SHAPE = np.dtype([("repetition_penalty", "<f4"), ("repetition_window", "<i4")])
+BIAS_MAX = 1e4   # largest |value| of a finite code bias
+
+
+def _clip_values(name, v, B):
+    """A per-clip value as a list of B elements (a length-B sequence, 1-D numpy array or 1-D tensor); a bool element, another
+    shape or another length raises ValueError."""
+    if torch.is_tensor(v) or isinstance(v, np.ndarray):
+        if v.ndim != 1:
+            raise ValueError("%s: per-clip values must be one-dimensional, got shape %s" % (name, tuple(v.shape)))
+        v = v.tolist()
+    v = list(v)
+    if len(v) != B:
+        raise ValueError("%s: %d per-clip values for %d clips" % (name, len(v), B))
+    for b, x in enumerate(v):
+        if isinstance(x, bool):
+            raise ValueError("%s: clip %d: a bool is not a shaping value, got %r" % (name, b, x))
+    return v
+
+
+def _check_shape_values(penalty, window):
+    """ValueError unless the repetition penalty is a number, finite and >= 1 in fp32, and the window an integer in
+    [1, 2^31 - 1]."""
+    try:
+        if isinstance(penalty, bool):
+            raise TypeError
+        with np.errstate(over="ignore"):
+            p32 = np.float32(float(penalty))
+    except (TypeError, ValueError):
+        raise ValueError("repetition_penalty must be a number, got %r" % (penalty,)) from None
+    if not (math.isfinite(p32) and p32 >= 1.0):
+        raise ValueError("repetition_penalty must be finite and >= 1 (1 = off), got %r" % (penalty,))
+    try:
+        if isinstance(window, bool) or int(window) != window:
+            raise TypeError
+    except (TypeError, ValueError):
+        raise ValueError("repetition_window must be an integer, got %r" % (window,)) from None
+    if not 1 <= int(window) <= 2 ** 31 - 1:
+        raise ValueError("repetition_window must lie in [1, 2^31 - 1] latent rows, got %r" % (window,))
+
+
+def check_clip_shape(repetition_penalty=1.0, repetition_window=8, B=None):
+    """Per-clip logit shaping as a host array [B] of ``CLIP_SHAPE`` (ts_clip_shape).  Each value is a scalar, broadcast to
+    every clip, or a length-B sequence / 1-D numpy array / 1-D tensor (B defaults to its length).  The penalty must be
+    finite and >= 1 in fp32 (1 = off), the window an integer >= 1 (latent rows).  A bool element, another shape or another
+    length raises ValueError; an element's error names its clip."""
+    cols = {}
+    for name, v in (("repetition_penalty", repetition_penalty), ("repetition_window", repetition_window)):
+        if _is_per_clip(v):
+            if B is None:
+                B = len(v)
+            cols[name] = _clip_values(name, v, B)
+    if B is None:
+        raise ValueError("check_clip_shape: no per-clip value and no batch size")
+    scalars = dict(repetition_penalty=repetition_penalty, repetition_window=repetition_window)
+    defaults = dict(repetition_penalty=1.0, repetition_window=8)
+    _check_shape_values(*(defaults[n] if n in cols else v for n, v in scalars.items()))   # the broadcast scalars
+    out = np.zeros(B, CLIP_SHAPE)
+    for b in range(B):
+        p, w = (cols[n][b] if n in cols else scalars[n] for n in ("repetition_penalty", "repetition_window"))
+        try:
+            _check_shape_values(p, w)
+        except ValueError as ex:
+            raise ValueError("clip %d: %s" % (b, ex)) from None
+        out[b] = (float(p), int(w))
+    return out
+
+
+def check_code_bias(code_bias, B):
+    """Code bias of a shaped call as a float32 tensor [B,2,2048] (host or device, as given): a float or integer tensor or
+    numpy array of shape [B,2,2048], or [2,2048] (the same two rows for every clip).  Column 0 biases the body codebook,
+    column 1 the hand codebook.  After conversion to float32 every value must be finite with |v| <= 1e4, or -inf (the code
+    is never drawn), and every (clip, column) row must keep a finite value.  Anything else raises ValueError naming the
+    clip and column.  The value check of a device tensor reads one reduction back: one synchronisation."""
+    if isinstance(code_bias, np.ndarray):
+        if code_bias.dtype.kind not in "fiu":
+            raise ValueError("code_bias must be a float array [%d,2,%d] or [2,%d], got dtype %s" % (B, NCODE, NCODE, code_bias.dtype))
+        code_bias = torch.from_numpy(np.ascontiguousarray(code_bias))
+    if not torch.is_tensor(code_bias):
+        raise ValueError("code_bias must be a float tensor or numpy array [%d,2,%d] or [2,%d], got %r"
+                         % (B, NCODE, NCODE, type(code_bias)))
+    if code_bias.dtype == torch.bool or code_bias.is_complex():
+        raise ValueError("code_bias must be a float tensor, got %s" % (code_bias.dtype,))
+    code_bias = code_bias.to(torch.float32)
+    if tuple(code_bias.shape) == (2, NCODE):
+        code_bias = code_bias.expand(B, 2, NCODE)
+    if tuple(code_bias.shape) != (B, 2, NCODE):
+        raise ValueError("code_bias must have shape [%d,2,%d] or [2,%d], got %s" % (B, NCODE, NCODE, tuple(code_bias.shape)))
+    code_bias = code_bias.contiguous()
+    fin = torch.isfinite(code_bias)
+    bad = torch.isnan(code_bias) | (code_bias == float("inf")) | (fin & (code_bias.abs() > BIAS_MAX))
+    flags = torch.stack([bad.any(-1), ~fin.any(-1)], -1).cpu()          # [B,2,2]: one read back
+    if flags.any():
+        b, c, k = (int(i) for i in torch.nonzero(flags)[0])
+        what = ("values must be finite with |v| <= %g, or -inf" % BIAS_MAX if k == 0
+                else "every code is -inf: the draw keeps no code")
+        raise ValueError("code_bias: clip %d, column %d (%s): %s" % (b, c, ("body", "hand")[c], what))
+    return code_bias
+
+
+def shaping_kwargs(repetition_penalty=1.0, repetition_window=8, code_bias=None, B=None):
+    """The shaping keywords a caller forwards to ``Engine.pixelcnn_generate`` / ``body_generate``: none when the call
+    shapes nothing (no code_bias, repetition_penalty 1 for every clip), so that such calls forward what they forwarded
+    before.  The penalty and window are validated here (``check_clip_shape``), the bias by the engine."""
+    shape = check_clip_shape(repetition_penalty, repetition_window, B)
+    if code_bias is None and not (shape["repetition_penalty"] != 1.0).any():
+        return {}
+    return dict(repetition_penalty=repetition_penalty, repetition_window=repetition_window, code_bias=code_bias)
+
+
 def sampled(temperature):
     """True when a call with this (validated) temperature draws noise: temperature > 0, for some clip when per clip."""
     if _is_per_clip(temperature):
@@ -420,7 +531,8 @@ class Engine:
         return out
 
     def pixelcnn_generate(self, aud, label, noise, T=None, pre_latents=None, want_logits=False, temperature=1.0, top_k=0,
-                          want_logp=False, top_p=1.0, min_p=0.0, want_kept=False, seeds=None, anchors=None, style=None):
+                          want_logp=False, top_p=1.0, min_p=0.0, want_kept=False, seeds=None, anchors=None, style=None,
+                          repetition_penalty=1.0, repetition_window=8, code_bias=None):
         """GatedPixelCNN.generate: aud [B,256,T0+T], label [B], noise [2T,B,2048] -> codes [B,T,2]
         (+ logits [2T,B,2048]).  Batches above the 64-sample tile are chunked here.
 
@@ -452,15 +564,25 @@ class Engine:
         (a length-B sequence, 1-D numpy array or 1-D tensor; ``check_clip_controls``), a scalar among them applying to every
         clip.  Clip b then draws exactly what it draws alone under its own values (ts_pixelcnn_sample_clips), whatever the
         other clips' values; a greedy clip reads no noise.  Sampling takes exactly one of noise and seeds when any clip has
-        temperature > 0.  All-scalar calls forward what they forwarded before."""
+        temperature > 0.  All-scalar calls forward what they forwarded before.
+
+        Logit shaping (ts_pixelcnn_sample_shaped; rule in include/talkshow_b200.h): ``repetition_penalty`` (theta >= 1,
+        1 = off) divides a positive logit by theta and multiplies a negative one by it for every code drawn at the same
+        column in the clip's previous ``repetition_window`` rows (prefix rows and pinned draws included); ``code_bias``
+        (``check_code_bias``: [2,2048] or [B,2,2048], -inf bans a code) is then added.  The controls act on the shaped
+        logits; logp stays that of the raw prior.  The penalty and window take a scalar or one value per clip
+        (``check_clip_shape``).  Without a bias and with theta 1 everywhere the call forwards what it forwarded before."""
         clip = None
         if per_clip(temperature, top_k, top_p, min_p):
             clip = check_clip_controls(temperature, top_k, top_p, min_p, aud.shape[0])
             ctl = _clip_source(clip, noise, seeds)
         else:
             ctl = _controlled(temperature, top_k, noise, want_logp, top_p, min_p, want_kept, seeds)
+        shape = check_clip_shape(repetition_penalty, repetition_window, aud.shape[0])
+        penalised = bool((shape["repetition_penalty"] != 1.0).any())
         aud = self._dev(aud, torch.float32)
         B = aud.shape[0]
+        bias = None if code_bias is None else self._dev(check_code_bias(code_bias, B), torch.float32)
         if label is None and style is None:
             raise ValueError("pixelcnn_generate: label is required without style")
         label = None if label is None else self._dev(label, torch.int64)
@@ -490,7 +612,17 @@ class Engine:
             kz = kept if (full or kept is None) else torch.empty(nb, T, 2, dtype=torch.int32, device=self.device)
             args = (self.h, _lib.ptr(aud[b0:b1].contiguous()), _lib.ptr(None if label is None else label[b0:b1].contiguous()), _lib.ptr(nz),
                     _lib.ptr(cz), _lib.ptr(lz), nb, T, _lib.ptr(None if pre is None else pre[b0:b1].contiguous()), T0)
-            if clip is not None:
+            if penalised or bias is not None:
+                c = (_ctl_struct(1.0, 0, 1.0, 0.0, pz, kz) if clip is not None
+                     else _ctl_struct(temperature, top_k, top_p, min_p, pz, kz))
+                args = args[:3] + (_lib.ptr(None if style is None else style[b0:b1]), self.pixelcnn_ncls, _lib.ptr(nz),
+                                   _lib.ptr(None if seeds is None else seeds[b0:b1]),
+                                   _lib.ptr(None if anchors is None else anchors[b0:b1])) + args[4:]
+                self._check(self.L.ts_pixelcnn_sample_shaped(*args, C.byref(c), None if clip is None else clip[b0:b1].ctypes.data,
+                                                             shape[b0:b1].ctypes.data if penalised else None,
+                                                             _lib.ptr(None if bias is None else bias[b0:b1]), self._s()),
+                            "ts_pixelcnn_sample_shaped")
+            elif clip is not None:
                 c = _ctl_struct(1.0, 0, 1.0, 0.0, pz, kz)      # logp / kept only: the draws' controls are clip[b0:b1]
                 args = args[:3] + (_lib.ptr(None if style is None else style[b0:b1]), self.pixelcnn_ncls, _lib.ptr(nz),
                                    _lib.ptr(None if seeds is None else seeds[b0:b1]),
@@ -665,7 +797,8 @@ class Engine:
         return out
 
     def body_generate(self, mfcc, label, noise, want_codes=True, temperature=1.0, top_k=0, want_logp=False, top_p=1.0,
-                      min_p=0.0, want_kept=False, seeds=None, anchors=None, style=None):
+                      min_p=0.0, want_kept=False, seeds=None, anchors=None, style=None, repetition_penalty=1.0,
+                      repetition_window=8, code_bias=None):
         """fused s2g_body_pixel core: mfcc [B,64,M] -> (codes [B,T,2], poses [B,4T,C]), C = 129 (258 for 6-D).
         Sampling controls as in ``pixelcnn_generate`` (ts_body_sample, ts_body_sample_ctl); ``want_logp`` appends logp
         [B,T,2], ``want_kept`` then kept [B,T,2] int32.  ``seeds`` [B] in place of ``noise``: seeded sampling
@@ -673,13 +806,17 @@ class Engine:
         (ts_body_sample_anchored; one synchronisation for a device tensor); the poses decode the resulting codes.
         ``style`` [B,T,ncls] or [B,ncls]: a speaker schedule as in ``pixelcnn_generate`` (ts_body_sample_styled; label
         may then be None).  Per-clip ``temperature`` / ``top_k`` / ``top_p`` / ``min_p`` as in ``pixelcnn_generate``
-        (ts_body_sample_clips); each clip's poses decode its own codes."""
+        (ts_body_sample_clips); each clip's poses decode its own codes.  ``repetition_penalty`` / ``repetition_window`` /
+        ``code_bias``: logit shaping as in ``pixelcnn_generate`` (ts_body_sample_shaped)."""
         clip = None
         if per_clip(temperature, top_k, top_p, min_p):
             clip = check_clip_controls(temperature, top_k, top_p, min_p, mfcc.shape[0])
             ctl = _clip_source(clip, noise, seeds)
         else:
             ctl = _controlled(temperature, top_k, noise, want_logp, top_p, min_p, want_kept, seeds)
+        shape = check_clip_shape(repetition_penalty, repetition_window, mfcc.shape[0])
+        penalised = bool((shape["repetition_penalty"] != 1.0).any())
+        bias = None if code_bias is None else self._dev(check_code_bias(code_bias, mfcc.shape[0]), torch.float32)
         mfcc = self._dev(mfcc, torch.float32)
         if label is None and style is None:
             raise ValueError("body_generate: label is required without style")
@@ -702,7 +839,17 @@ class Engine:
             nz = noise if (full or noise is None) else noise[:, b0:b1].contiguous()
             args = (self.h, _lib.ptr(mfcc[b0:b1]), _lib.ptr(None if label is None else label[b0:b1]), _lib.ptr(nz),
                     _lib.ptr(None if codes is None else codes[b0:b1]), _lib.ptr(poses[b0:b1]), b1 - b0, M)
-            if clip is not None:
+            if penalised or bias is not None:
+                lz, kz = None if logp is None else logp[b0:b1], None if kept is None else kept[b0:b1]
+                c = _ctl_struct(1.0, 0, 1.0, 0.0, lz, kz) if clip is not None else _ctl_struct(temperature, top_k, top_p, min_p, lz, kz)
+                args = args[:3] + (_lib.ptr(None if style is None else style[b0:b1]), self.pixelcnn_ncls, _lib.ptr(nz),
+                                   _lib.ptr(None if seeds is None else seeds[b0:b1]),
+                                   _lib.ptr(None if anchors is None else anchors[b0:b1])) + args[4:]
+                self._check(self.L.ts_body_sample_shaped(*args, C.byref(c), None if clip is None else clip[b0:b1].ctypes.data,
+                                                         shape[b0:b1].ctypes.data if penalised else None,
+                                                         _lib.ptr(None if bias is None else bias[b0:b1]), self._s()),
+                            "ts_body_sample_shaped")
+            elif clip is not None:
                 c = _ctl_struct(1.0, 0, 1.0, 0.0, None if logp is None else logp[b0:b1], None if kept is None else kept[b0:b1])
                 args = args[:3] + (_lib.ptr(None if style is None else style[b0:b1]), self.pixelcnn_ncls, _lib.ptr(nz),
                                    _lib.ptr(None if seeds is None else seeds[b0:b1]),

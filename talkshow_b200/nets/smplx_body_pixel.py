@@ -10,7 +10,8 @@ import torch
 
 from ..data_utils.lower_body import c_index_3d, c_index_6d
 from ..data_utils.utils import get_mfcc_sepa, get_mfcc_ta, load_wav
-from ..engine import check_clip_controls, check_sample_controls, check_style, per_clip, resolve_clip_seeds, sample_controls, sampled
+from ..engine import (check_clip_controls, check_sample_controls, check_style, per_clip, resolve_clip_seeds, sample_controls,
+                      sampled, shaping_kwargs)
 from .base import draw_sampler_noise, resolve_device, shared_engine, strip_module
 
 
@@ -110,7 +111,8 @@ class TrainWrapper:
                        continuity=False, id=None, fps=15, sr=22000, B=1, am=None, am_sr=None, frame=0, **kwargs):
         """(aud_fn) -> generated motion, numpy (B, F, 129).  Reference: :232-289."""
         assert self.args.infer, "train mode"
-        ctl = {k: kwargs[k] for k in ("temperature", "top_k", "keep_logp", "top_p", "min_p", "clip_seeds") if k in kwargs}
+        ctl = {k: kwargs[k] for k in ("temperature", "top_k", "keep_logp", "top_p", "min_p", "clip_seeds", "repetition_penalty",
+                                      "repetition_window", "code_bias") if k in kwargs}
         if kwargs.get("noise_fn") is not None and kwargs.get("clip_seeds") is not None:
             raise ValueError("infer_on_audio: noise_fn and clip_seeds are two noise sources; give one")
         if kwargs.get("anchors") is not None:
@@ -135,7 +137,7 @@ class TrainWrapper:
         return self.generate(mfcc, label, noise_fn=kwargs.get("noise_fn"), **ctl).cpu().numpy()
 
     def generate(self, aud, id, frame_num=0, noise_fn=None, temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0,
-                 clip_seeds=None, anchors=None, style=None):
+                 clip_seeds=None, anchors=None, style=None, repetition_penalty=1.0, repetition_window=8, code_bias=None):
         """tensor API (:306-326): aud [B,64,M] features, id [B] -> torch (B, F, 129) on the device.
         (The reference's version passes decode()'s tuple to torch.cat and raises; this returns the
         tensor its infer_on_audio builds.)
@@ -161,13 +163,20 @@ class TrainWrapper:
 
         Per-clip controls: ``temperature``, ``top_k``, ``top_p`` and ``min_p`` each take a scalar or one value per clip (a
         length-B sequence, 1-D array or tensor; Engine.pixelcnn_generate), so one batch serves clips with different
-        settings; clip b draws what it draws alone under its own values.  Noise is drawn when any clip samples."""
+        settings; clip b draws what it draws alone under its own values.  Noise is drawn when any clip samples.
+
+        Logit shaping (Engine.pixelcnn_generate): ``repetition_penalty`` (>= 1, 1 = off; scalar or per clip) penalises the
+        codes the clip drew at the same column in its last ``repetition_window`` latent rows (8 rows, about 1 s), which
+        breaks the loops greedy or cold sampling falls into; ``code_bias`` [2,2048] or [B,2,2048] is added to the logits
+        (column 0 body codes, column 1 hand codes; -inf never draws the code)."""
         mfcc = aud.to(torch.float32)
         B, _, M = mfcc.shape
         T = self.engine.latent_rows(M)
         seeds = self._seeds(clip_seeds, B, noise_fn)
+        shaping = shaping_kwargs(repetition_penalty, repetition_window, code_bias, B)
         noise = self._draw_noise(T, B, noise_fn, temperature, top_k, top_p, min_p, seeds)
         ctl = sample_controls(temperature, top_k, keep_logp, top_p, min_p)
+        ctl.update(shaping)
         if noise is None and seeds is not None and sampled(temperature):
             ctl["seeds"] = seeds
         if anchors is not None:
@@ -199,7 +208,8 @@ class TrainWrapper:
         return resolve_clip_seeds(clip_seeds, B)
 
     def infer(self, aud_feat, frame, id, B, pre_latents=None, pre_audio=None, pre_pose=None, noise_fn=None,
-              temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None, anchors=None, style=None):
+              temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None, anchors=None, style=None,
+              repetition_penalty=1.0, repetition_window=8, code_bias=None):
         """The reference's inner call (:291-304): aud_feat [B,M,64] (time-major features of ONE chunk) ->
         (latents [B,T,2], audio [B,256,T,2], body [B,39,4T], hand [B,90,4T]).  ``pre_latents`` / ``pre_audio`` (the first
         two results of the previous chunk's call) condition the sampler on that chunk (GatedPixelCNN.generate :158-165);
@@ -210,13 +220,16 @@ class TrainWrapper:
         the T0 rows of the previous chunk), so a seeded clip's noise does not depend on where it is cut into chunks.
         ``anchors`` [B,T,2] cover this chunk's T rows (as in ``generate``); with ``pre_latents`` they pin rows after the
         prefix.  ``style`` [B,T0+T,4] (or [B,4]) as in ``generate``, its rows covering the prefix and the chunk.  Per-clip
-        controls as in ``generate``."""
+        controls and logit shaping as in ``generate``; with ``pre_latents`` the repetition window reaches back into the
+        prefix's codes."""
         a = self.engine.audio_encode(aud_feat.transpose(1, 2).contiguous())            # [B,256,T]
         T = a.shape[2]
         label = id.reshape(-1)
         seeds = self._seeds(clip_seeds, B, noise_fn)
+        shaping = shaping_kwargs(repetition_penalty, repetition_window, code_bias, B)
         noise = self._draw_noise(T, B, noise_fn, temperature, top_k, top_p, min_p, seeds)
         ctl = sample_controls(temperature, top_k, keep_logp, top_p, min_p)
+        ctl.update(shaping)
         if noise is None and seeds is not None and sampled(temperature):
             ctl["seeds"] = seeds
         if anchors is not None:

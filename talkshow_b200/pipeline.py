@@ -10,7 +10,8 @@ from __future__ import annotations
 
 import torch
 
-from .engine import Engine, check_anchors, check_clip_controls, check_style, per_clip, resolve_clip_seeds, sample_controls, sampled
+from .engine import (Engine, check_anchors, check_clip_controls, check_clip_shape, check_code_bias, check_style, per_clip,
+                     resolve_clip_seeds, sample_controls, sampled, shaping_kwargs)
 from .nets.base import draw_sampler_noise
 
 
@@ -78,7 +79,8 @@ class WholeBody:
             self.e2 = None
 
     def generate(self, mfcc, wave, label, noise=None, stand=False, per_step_noise=True, temperature=1.0, top_k=0,
-                 keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None, anchors=None, keep_codes=False, style=None):
+                 keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None, anchors=None, keep_codes=False, style=None,
+                 repetition_penalty=1.0, repetition_window=8, code_bias=None):
         """mfcc [B,64,M], wave [B,N] (16 kHz), label [B] on the device -> poses [B,F,265] (device).
         F = N*30//16000 face frames; the body (4*T frames) is padded/truncated to F like demo.py:207-211.
         Sampling controls of the body prior as in s2g_body_pixel.generate: ``temperature`` (0 = greedy, no noise is
@@ -93,11 +95,15 @@ class WholeBody:
         not read.  The face path keeps the demo's zero id (demo.py:173-181) whatever the style: the body prior is the only
         net styled here (s2g_face.generate_ids takes a soft id for the face).
         ``temperature`` / ``top_k`` / ``top_p`` / ``min_p`` may each be given per clip (s2g_body_pixel.generate): one batch
-        serves clips with different settings, on the overlapped and the sequential path alike."""
+        serves clips with different settings, on the overlapped and the sequential path alike.
+        ``repetition_penalty`` / ``repetition_window`` / ``code_bias``: logit shaping of the body prior
+        (s2g_body_pixel.generate), on both paths."""
         B, _, M = mfcc.shape
         frame = wave.shape[1] * 30 // 16000
         T = self.e.latent_rows(M)
+        shaping = shaping_kwargs(repetition_penalty, repetition_window, code_bias, B)
         ctl = sample_controls(temperature, top_k, keep_logp, top_p, min_p)
+        ctl.update(shaping)
         want_kept = bool(ctl.get("want_kept"))
         if noise is not None and clip_seeds is not None:
             raise ValueError("WholeBody.generate: noise and clip_seeds are two noise sources; give one")
@@ -131,7 +137,7 @@ class WholeBody:
                 self.last_kept.record_stream(cur)
             if keep_codes:
                 self.last_codes.record_stream(cur)
-            for t in (mfcc, label, noise, ctl.get("seeds"), ctl.get("anchors"), ctl.get("style")):
+            for t in (mfcc, label, noise, ctl.get("seeds"), ctl.get("anchors"), ctl.get("style"), ctl.get("code_bias")):
                 if torch.is_tensor(t) and t.is_cuda:
                     t.record_stream(self._side)                          # allocated here, consumed on the side stream
             return self.e.assemble_pose(face, body, stand)
@@ -178,7 +184,7 @@ class WholeBody:
 
     def generate_sharded(self, mfcc, wave, label, rank, world, noise_full=None, seed=None, stand=False, gather=True,
                          group=None, temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None,
-                         anchors=None, style=None):
+                         anchors=None, style=None, repetition_penalty=1.0, repetition_window=8, code_bias=None):
         """Multi-GPU form of ``generate`` whose RESULT DOES NOT DEPEND ON ``world`` (SURVEY.md §8e): the arguments are
         the FULL batch (host or device tensors, identical on every rank), the sampler noise is drawn for the full batch in
         the reference's order — ``noise_full`` [2T,B,2048], or drawn here from ``seed`` on this rank's device generator
@@ -192,7 +198,9 @@ class WholeBody:
         ``anchors`` [B,T,2] (as in ``generate``, for the full batch): rank r passes the rows of its shard, so the gathered
         result equals ``generate`` with the same anchors on one GPU.  ``style`` [B,T,ncls] or [B,ncls] (full batch, as in
         ``generate``): rank r passes its shard's rows.  Per-clip ``temperature`` / ``top_k`` / ``top_p`` / ``min_p`` (full
-        batch, as in ``generate``): rank r passes its shard's values."""
+        batch, as in ``generate``): rank r passes its shard's values.  ``repetition_penalty`` / ``repetition_window`` (scalar
+        or per clip) and ``code_bias`` ([2,2048] or [B,2,2048]) as in ``generate``: rank r passes its shard's values and bias
+        rows."""
         B, _, M = mfcc.shape
         lo, hi = shard_range(B, rank, world)
         T = self.e.latent_rows(M)
@@ -211,6 +219,11 @@ class WholeBody:
             ctl["anchors"] = check_anchors(anchors, B, T)[lo:hi]
         if style is not None:
             ctl["style"] = check_style(style, B, T, self.e.pixelcnn_ncls)[lo:hi]
+        if shaping_kwargs(repetition_penalty, repetition_window, code_bias, B):
+            shape = check_clip_shape(repetition_penalty, repetition_window, B)[lo:hi]
+            ctl.update(repetition_penalty=shape["repetition_penalty"], repetition_window=shape["repetition_window"])
+            if code_bias is not None:
+                ctl["code_bias"] = check_code_bias(code_bias, B)[lo:hi]
         if seeds is not None:
             ctl["clip_seeds"] = seeds[lo:hi]
         elif noise_full is None and sampled(temperature):
