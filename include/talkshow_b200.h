@@ -257,6 +257,38 @@ int ts_pixelcnn_sample_shaped(ts_engine* e, const float* aud, const int64_t* lab
                               float* logits_out, int B, int T, const int64_t* pre_latents, int T0, const ts_sample_ctl* ctl,
                               const ts_clip_ctl* clip_ctl, const ts_clip_shape* clip_shape, const float* code_bias,
                               void* stream);
+/* ---- guided sampling: each draw pushed away from a negative conditioning ------------------------------------------------
+ * A guided call has P pairs.  Pair p has two branches: branch 2p is the clip (conditional), branch 2p + 1 its negative
+ * conditioning (silence, another speaker, a style blend: the prior was trained without condition dropout, so this is
+ * contrastive guidance, not classifier-free guidance against a learned unconditional model).
+ *  - Conditioning is per branch (2P rows): aud [2P,256,T0+T], label [2P], style [2P,T0+T,ncls].
+ *  - Draw inputs are per pair (P rows): noise [2T,P,2048] or seeds [P], clip_ctl [P], clip_shape [P], code_bias [P,2,2048],
+ *    anchors [P,T,2], pre_latents [P,T0,2] (motion, fed to both branches) and guidance [P] (HOST memory).
+ *  - Outputs are per branch (2P rows): idx_out [2P,T,2], logits_out [2T,2P,2048], ctl->logp_out / ctl->kept_out [2P,T,2].
+ * For the draw at row r, column c of pair p:
+ *  1. l_c, l_u = the raw logits of branches 2p and 2p + 1; with s = w_p - 1 (fp32 subtraction),
+ *     g_n = l_c,n + s * (l_c,n - l_u,n) as three separately rounded fp32 operations (subtract, multiply, add; no
+ *     contraction).  At w = 1, g = l_c (up to the sign of a zero, which the draw does not see).
+ *  2. The pair's shaping (ts_pixelcnn_sample_shaped: penalty over the pair's history, then the bias) acts on g, then the
+ *     pair's controls (temperature, top_k, top_p, min_p, greedy, the overflow fallback) with the pair's noise or seed.
+ *  3. Both branches write the code to their idx_out rows and feed it to their own next rows: later draws of both branches
+ *     see the guided code.
+ *  4. logp_out of each branch is the log p of the code under that branch's raw prior (branch 2p: the conditional log p of
+ *     every sampling call; branch 2p + 1: the negative one).  kept_out is the guided keep-set size, equal in both rows.
+ *  5. A pinned draw (anchors[p]) pins both branches and is not guided.
+ *  6. w must be finite and in [0, TS_GUIDANCE_MAX] (TS_ERR_INVALID, the message names the pair).  Whatever the logits,
+ *     the code lies in [0, 2048).
+ * Contract: a pair with w = 1 draws, bit for bit, the codes, conditional log p and kept sizes of ts_pixelcnn_sample_shaped
+ * run on its conditional branch alone with the same draw inputs; a pair's results do not depend on the other pairs; a
+ * seeded pair's q is keyed by (seed, row, column, code) as in ts_pixelcnn_sample_seeded.  The grid-wide executor takes at
+ * most 64 branches (32 pairs) per call; the cluster executor any number.  TS_ERR_INVALID: P < 1, guidance NULL or a bad
+ * w, or anything ts_pixelcnn_sample_shaped refuses. */
+#define TS_GUIDANCE_MAX 100.0f
+int ts_pixelcnn_sample_guided(ts_engine* e, const float* aud, const int64_t* label, const float* style, int ncls,
+                              const float* noise, const int64_t* seeds, const int64_t* anchors, int64_t* idx_out,
+                              float* logits_out, int P, int T, const int64_t* pre_latents, int T0, const ts_sample_ctl* ctl,
+                              const ts_clip_ctl* clip_ctl, const ts_clip_shape* clip_shape, const float* code_bias,
+                              const float* guidance, void* stream);
 /* GatedPixelCNN.forward (teacher forced), :130-150, for rows [0,T): logits_out [B,2048,T,2]. */
 int ts_pixelcnn_logits(ts_engine* e, const float* aud, const int64_t* label, const int64_t* codes,
                        float* logits_out, int B, int T, void* stream);
@@ -359,6 +391,13 @@ int ts_body_sample_shaped(ts_engine* e, const float* mfcc, const int64_t* label,
                           const float* noise, const int64_t* seeds, const int64_t* anchors, int64_t* codes, float* poses,
                           int B, int M, const ts_sample_ctl* ctl, const ts_clip_ctl* clip_ctl,
                           const ts_clip_shape* clip_shape, const float* code_bias, void* stream);
+/* ts_body_sample_shaped under the guidance of ts_pixelcnn_sample_guided: mfcc [2P,64,M], label / style per branch, every
+ * draw input per pair, guidance [P] (HOST).  codes [2P,T,2] (may be NULL) gets every branch's codes (both rows of a pair
+ * equal); poses [P,4T,C] decodes the conditional branches only. */
+int ts_body_sample_guided(ts_engine* e, const float* mfcc, const int64_t* label, const float* style, int ncls,
+                          const float* noise, const int64_t* seeds, const int64_t* anchors, int64_t* codes, float* poses,
+                          int P, int M, const ts_sample_ctl* ctl, const ts_clip_ctl* clip_ctl,
+                          const ts_clip_shape* clip_shape, const float* code_bias, const float* guidance, void* stream);
 
 /* Audio front-end of get_mfcc_ta, data_utils/utils.py:148-177 (SURVEY.md §8f-1): wave [B,N] mono at
  * `sr` Hz -> torchaudio Resample(sr, 22000) -> MFCC(64 coefficients, n_fft 2048, hop 734 = 30 fps, 256 HTK

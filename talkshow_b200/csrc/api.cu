@@ -1,5 +1,6 @@
 // talkshow_b200 — engine lifetime, error reporting, pose assembly, fused body path entry.
 #include "convstack.h"
+#include <climits>
 #include "pixelcnn.h"
 
 using namespace ts;
@@ -243,11 +244,12 @@ extern "C" int ts_vq_dim(ts_engine* e, int which) {
 // seeds (ts_body_sample_seeded): per-clip seeds in place of noise.  anchors (ts_body_sample_anchored): pinned draws.
 // style (ts_body_sample_styled): per-row speaker weights in place of label.  clip_ctl (ts_body_sample_clips): per-clip
 // controls (host, validated) in place of ctl's four.  clip_shape / code_bias (ts_body_sample_shaped): logit shaping.
+// guide (ts_body_sample_guided): B = 2P branches sampled in pairs; codes gets every branch, poses the P conditional ones.
 static void body_generate(ts_engine* e, const float* mfcc, const int64_t* label, const float* noise, int64_t* codes,
                           float* poses, int B, int M, void* stream, const SampleCtl* ctl, const int64_t* seeds = nullptr,
                           const int64_t* anchors = nullptr, const float* style = nullptr,
                           const ts_clip_ctl* clip_ctl = nullptr, const ts_clip_shape* clip_shape = nullptr,
-                          const float* code_bias = nullptr) {
+                          const float* code_bias = nullptr, const float* guide = nullptr) {
   ts::require_device(e);
   if (!e->conv || !e->conv->audio_loaded) fail(TS_ERR_NOT_LOADED, "audio encoder weights not loaded");
   if (!e->conv->vq[0].loaded || !e->conv->vq[1].loaded) fail(TS_ERR_NOT_LOADED, "vq weights not loaded");
@@ -265,13 +267,15 @@ static void body_generate(ts_engine* e, const float* mfcc, const int64_t* label,
     int64_t* idx = e->ws.alloc<int64_t>((size_t)B * T * 2);
     int64_t* idx_c = e->ws.alloc<int64_t>((size_t)B * T * 2);  // [2][B][T] column-split copy
     pixelcnn_generate_act(e, a, label, noise, idx, nullptr, B, T, nullptr, 0, s, false, ctl, seeds, anchors, style, clip_ctl,
-                          clip_shape, code_bias);
-    split_codes(e, idx, idx_c, B, T, codes, s);
+                          clip_shape, code_bias, guide);
+    if (guide) split_guided_codes(e, idx, idx_c, B / 2, T, codes, s);   // decode the conditional branches only
+    else split_codes(e, idx, idx_c, B, T, codes, s);
+    const int Bd = guide ? B / 2 : B;
     const int c0 = e->conv->vq[0].out_dim, c1 = e->conv->vq[1].out_dim;   // 39 + 90 (axis-angle) or 78 + 180 (6-D)
     // Small batches: each decoder is a chain of ~20 launches that fill a few SMs, so the hand decoder runs on a second
     // stream beside the body decoder (fork after the code split, join before the call returns to the caller's stream).
     // The two chains share nothing but their input codes: separate workspace blocks, disjoint columns of `poses`.
-    const bool par = !e->ws.sizing && B <= e->vq_parallel_batch;
+    const bool par = !e->ws.sizing && Bd <= e->vq_parallel_batch;
     if (par) {
       if (!e->aux_stream) {
         int prio = 0;
@@ -285,7 +289,7 @@ static void body_generate(ts_engine* e, const float* mfcc, const int64_t* label,
     }
     for (int w = 0; w < 2; ++w) {
       cudaStream_t sw = (w == 1 && par) ? e->aux_stream : s;
-      Act3 y = run_vq_decode(e, e->conv->vq[w], idx_c + (size_t)w * B * T, B, T, sw);
+      Act3 y = run_vq_decode(e, e->conv->vq[w], idx_c + (size_t)w * Bd * T, Bd, T, sw);
       act_to_btc(e, y, e->conv->vq[w].out_dim, poses, c0 + c1, w ? c0 : 0, sw);
     }
     if (par) {
@@ -402,5 +406,23 @@ extern "C" int ts_body_sample_shaped(ts_engine* e, const float* mfcc, const int6
   if (clip_shape) check_clip_shape(clip_shape, B, "ts_body_sample_shaped");
   const SampleCtl c = shaped_ctl(ctl, clip_ctl, B, noise, seeds, "ts_body_sample_shaped");
   body_generate(e, mfcc, label, noise, codes, poses, B, M, stream, &c, seeds, anchors, style, clip_ctl, clip_shape, code_bias);
+  TS_API_END(e)
+}
+
+extern "C" int ts_body_sample_guided(ts_engine* e, const float* mfcc, const int64_t* label, const float* style, int ncls,
+                                     const float* noise, const int64_t* seeds, const int64_t* anchors, int64_t* codes,
+                                     float* poses, int P, int M, const ts_sample_ctl* ctl, const ts_clip_ctl* clip_ctl,
+                                     const ts_clip_shape* clip_shape, const float* code_bias, const float* guidance,
+                                     void* stream) {
+  TS_API_BEGIN(e)
+  ts::require_device(e);
+  if (!e->pix) fail(TS_ERR_NOT_LOADED, "pixelcnn weights not loaded");
+  if (P < 1 || P > INT_MAX / 2) fail(TS_ERR_INVALID, "ts_body_sample_guided: P=%d pairs", P);
+  check_style(e, label, style, ncls, "ts_body_sample_guided");
+  check_guidance(guidance, P, "ts_body_sample_guided");
+  if (clip_shape) check_clip_shape(clip_shape, P, "ts_body_sample_guided");
+  const SampleCtl c = shaped_ctl(ctl, clip_ctl, P, noise, seeds, "ts_body_sample_guided");
+  body_generate(e, mfcc, label, noise, codes, poses, 2 * P, M, stream, &c, seeds, anchors, style, clip_ctl, clip_shape,
+                code_bias, guidance);
   TS_API_END(e)
 }

@@ -15,6 +15,7 @@
 #include "convstack.h"
 
 #include <algorithm>
+#include <climits>
 #include <memory>
 #include <cmath>
 
@@ -488,7 +489,17 @@ struct PixArgs {
   // repetition penalty and window, or null (theta 1); [B][2][2048] (device) code bias, or null
   const ts_clip_shape* clip_shape;
   const float* code_bias;
+  // guided sampling (ts_pixelcnn_sample_guided), read by the WARP instantiations only: [B / 2] (device) guidance scale of
+  // each pair of samples (2p conditional, 2p + 1 negative); every draw input above is then indexed by the pair; or null
+  const float* guide;
 };
+
+// The draw-input index of sample m (WARP instantiations only): in a guided call samples 2p and 2p + 1 are the two branches
+// of pair p and read pair p's noise or seed, controls, anchors, shaping and scale; otherwise sample m's own.
+template <class Args>
+__device__ __forceinline__ int draw_index(const Args& A, int m) {
+  return A.guide ? m >> 1 : m;
+}
 
 // The sampling controls of clip m (global index): its entry of A.clip_ctl, else the call's scalar controls.  Every draw
 // of one clip runs in one CTA, so the value is uniform over the threads that call draw_controlled together.
@@ -534,10 +545,12 @@ __device__ __forceinline__ ShapeCtl shape_ctl(const Args& A, int m) {
 // clip m: coherent L2 loads, never the read-only path) and the bias row.  Everything it reads is final before the sample
 // stage starts, so both persistent executors stage it before their barrier wait, where it overlaps the wait; the bitmap is
 // published by the caller's next barrier.  Out-of-range history codes are skipped.  Uniform over the CTA (one clip).
+// Guided: theta, W and the bias row are the pair's (draw_index); the history is the branch's own, which holds the pair's
+// codes (both branches write every guided code, and the host gives each branch a copy of the pair's pre rows).
 template <class Args, class Bar>
 __device__ __forceinline__ void shape_stage(const Args& A, int m, int r, int c, float* red, Bar bar) {
   const int tid = threadIdx.x;
-  const ShapeCtl sc = shape_ctl(A, m);
+  const ShapeCtl sc = shape_ctl(A, draw_index(A, m));
   if (sc.theta != 1.f) {
     unsigned* bits = reinterpret_cast<unsigned*>(red + SHAPE_BITS);
     if (tid < PIX_NCODE / 32) bits[tid] = 0u;
@@ -551,18 +564,19 @@ __device__ __forceinline__ void shape_stage(const Args& A, int m, int r, int c, 
     }
   }
   if (A.code_bias) {
-    const float* b = A.code_bias + ((size_t)m * 2 + c) * PIX_NCODE;
+    const float* b = A.code_bias + ((size_t)draw_index(A, m) * 2 + c) * PIX_NCODE;
 #pragma unroll
     for (int j = 0; j < 8; ++j) red[SHAPE_BIAS + tid + 256 * j] = __ldg(b + tid + 256 * j);
   }
 }
 
 // Shapes the raw logits l of clip m's draw in place from what shape_stage staged: the penalty on the history's codes,
-// then the bias.  Returns whether the draw is shaped (theta != 1 or a bias), the same in every thread.
+// then the bias.  Returns whether the draw is shaped (theta != 1 or a bias), the same in every thread.  Guided: the pair's
+// theta (draw_index).
 template <class Args>
 __device__ __forceinline__ bool shape_logits(const Args& A, int m, const float* red, float (&l)[8]) {
   const int tid = threadIdx.x;
-  const ShapeCtl sc = shape_ctl(A, m);
+  const ShapeCtl sc = shape_ctl(A, draw_index(A, m));
   if (sc.theta != 1.f) {
     const unsigned* bits = reinterpret_cast<const unsigned*>(red + SHAPE_BITS);
 #pragma unroll
@@ -1464,6 +1478,42 @@ __device__ __forceinline__ void draw_noise(const Args& A, int r, int c, int m, f
     for (int j = 0; j < 8; ++j) q[j] = __ldcs(src + tid + 256 * j);
   }
 }
+// draw_noise of the WARP kernels: a guided call's pair p = m >> 1 (draw_index) reads seeds[p], or column p of noise
+// [2T][B / 2][2048]; every other call is draw_noise.
+template <bool WARP, class Args>
+__device__ __forceinline__ void draw_noise_of(const Args& A, int r, int c, int m, float (&q)[8]) {
+  if constexpr (WARP) {
+    if (A.guide) {
+      const int tid = threadIdx.x, p = m >> 1;
+      if (A.seeds) {
+        seeded_q(A.seeds[p], r, c, tid, q);
+      } else {
+        const float* src = A.noise + ((size_t)(2 * (r - A.T0) + c) * (A.B >> 1) + p) * PIX_NCODE;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) q[j] = __ldcs(src + tid + 256 * j);
+      }
+      return;
+    }
+  }
+  draw_noise(A, r, c, m, q);
+}
+
+// The guided logits of branch m's draw (ts_pixelcnn_sample_guided), in place of its raw logits l: with l_c the raw logits
+// of branch 2p (the conditional one, p = m >> 1), l_u those of branch 2p + 1 and s = w_p - 1, g = l_c + s (l_c - l_u) in
+// three separately rounded fp32 operations.  l holds branch m's raw logits; `partner` points at code 0 of branch m ^ 1's
+// LOG slot, `stride` floats between codes.  Both branches of a pair compute the same g from the same two slots, so they
+// draw the same code with no exchange.  Every slot is final: the sample stage follows the barrier after the logits stage.
+template <class Args>
+__device__ __forceinline__ void guide_logits(const Args& A, int m, const float* partner, int stride, float (&l)[8]) {
+  const int tid = threadIdx.x;
+  const float s = __fsub_rn(__ldg(A.guide + (m >> 1)), 1.f);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float o = __ldcg(partner + (size_t)(tid + 256 * j) * stride);
+    const float lc = (m & 1) ? o : l[j], lu = (m & 1) ? l[j] : o;
+    l[j] = __fadd_rn(lc, __fmul_rn(s, __fsub_rn(lc, lu)));
+  }
+}
 
 // softmax over 2048 logits + categorical draw = argmax(p / q) (ATen multinomial, num_samples = 1),
 // then embedding gather of the sampled code into the E ring.  One CTA per sample.
@@ -1494,26 +1544,28 @@ __device__ void run_sample_task(const PixTask& t, const PixArgs& A, int r, int m
   if constexpr (WARP) {
     if (!forced) {
       const size_t at = ((size_t)m * (A.Ttot - A.T0) + (r - A.T0)) * 2 + c;
-      const long long pin = anchor_of(A, at);   // the same in every thread: a uniform branch
+      const int d = draw_index(A, m);   // m, or a guided call's pair
+      const long long pin = anchor_of(A, ((size_t)d * (A.Ttot - A.T0) + (r - A.T0)) * 2 + c);   // uniform branch
       if (pin >= 0) {
         code = pin;
         draw_pinned(l, code, red, A.logp_out ? A.logp_out + at : nullptr, A.kept_out ? A.kept_out + at : nullptr, CtaBar());
       } else {
-        const DrawCtl dc = draw_ctl(A, m);   // clip m's controls: the whole CTA serves clip m
+        const DrawCtl dc = draw_ctl(A, d);   // clip m's (pair d's) controls: the whole CTA serves clip m
         float qv[8];
         if (dc.temperature > 0.f) {
           if (QPRE) {
 #pragma unroll
             for (int j = 0; j < 8; ++j) qv[j] = qpre[j];
           } else {
-            draw_noise(A, r, c, m, qv);
+            draw_noise_of<true>(A, r, c, m, qv);
           }
         }
-        const bool shaped = shape_logits(A, m, red, l);
+        if (A.guide) guide_logits(A, m, A.arena + A.lay.LOG + (m ^ 1), MB, l);
+        const bool shaped = shape_logits(A, m, red, l) || A.guide;
         float* logp = A.logp_out ? A.logp_out + at : nullptr;
         code = draw_controlled(l, qv, dc.temperature, dc.top_k, dc.top_p, dc.min_p, red, shaped ? nullptr : logp,
                                A.kept_out ? A.kept_out + at : nullptr, CtaBar());
-        if (shaped && logp) {   // log p under the raw prior: the LOG slot still holds the unshaped logits
+        if (shaped && logp) {   // log p under the branch's raw prior: the LOG slot still holds its unshaped logits
 #pragma unroll
           for (int j = 0; j < 8; ++j) l[j] = __ldcg(A.arena + A.lay.LOG + ax<MB>(tid + 256 * j, m));
           draw_pinned(l, code, red, logp, nullptr, CtaBar());
@@ -1688,8 +1740,8 @@ __global__ void __launch_bounds__(PIX_THREADS, 1) pixelcnn_kernel(PixArgs A, int
     // the sampler noise of this position is an input of the call (or, seeded, a function of the seed and the position):
     // loaded / computed before the barrier wait, so it overlaps the wait
     float qpre[8];
-    if (active && t.epi == EPI_SAMPLE && cta < A.B && r >= A.T0 && (!WARP || draw_temperature(A, cta) > 0.f))   // greedy: no noise
-      draw_noise(A, r, t.col, cta, qpre);
+    if (active && t.epi == EPI_SAMPLE && cta < A.B && r >= A.T0 && (!WARP || draw_temperature(A, draw_index(A, cta)) > 0.f))
+      draw_noise_of<WARP>(A, r, t.col, cta, qpre);   // greedy: no noise
     if constexpr (WARP) {   // the shaping inputs of this draw (ts_pixelcnn_sample_shaped), likewise before the wait
       if (active && t.epi == EPI_SAMPLE && cta < A.B && r >= A.T0 && (A.clip_shape || A.code_bias))
         shape_stage(A, cta, r, t.col, red, CtaBar());
@@ -1747,6 +1799,28 @@ void split_codes(ts_engine* e, const int64_t* idx, int64_t* idx_c, int B, int T,
   TS_CUDA(cudaGetLastError());
 }
 
+// one thread per (branch, row): every branch's codes to codes_out, the conditional branches' (2p) to idx_c [2][P][T]
+__global__ void split_guided_codes_kernel(const int64_t* __restrict__ idx, int64_t* __restrict__ idx_c, int64_t* codes_out,
+                                          int P, int T) {
+  const int n = 2 * P * T;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const int64_t a = idx[2 * i], b = idx[2 * i + 1];
+    const int br = i / T, t = i - br * T;
+    if ((br & 1) == 0) {
+      const int j = (br >> 1) * T + t;
+      idx_c[j] = a;
+      idx_c[(size_t)P * T + j] = b;
+    }
+    if (codes_out) { codes_out[2 * i] = a; codes_out[2 * i + 1] = b; }
+  }
+}
+void split_guided_codes(ts_engine* e, const int64_t* idx, int64_t* idx_c, int P, int T, int64_t* codes_out, cudaStream_t s) {
+  if (e->ws.sizing) return;
+  split_guided_codes_kernel<<<cdiv(2 * P * T, 256), 256, 0, s>>>(idx, idx_c, codes_out, P, T);
+  e->launches++;
+  TS_CUDA(cudaGetLastError());
+}
+
 // logits [2T][B][2048] (step-major) -> [B][2048][T][2]
 __global__ void logits_to_ref_kernel(const float* __restrict__ in, float* __restrict__ out, int B, int T) {
   long n = (long)2 * T * B * PIX_NCODE;
@@ -1763,7 +1837,7 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
                            int64_t* idx_out, float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s,
                            bool logits_all, const SampleCtl* ctl, const int64_t* seeds, const int64_t* anchors,
                            const float* style, const ts_clip_ctl* clip_ctl, const ts_clip_shape* clip_shape,
-                           const float* code_bias) {
+                           const float* code_bias, const float* guide) {
   PixelPlan* P = e->pix;
   Plan3* Q = (Plan3*)P->p3;
   const int Ttot = T0 + T, D = P->D;
@@ -1791,7 +1865,7 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
 
   if (v3) {   // cluster-resident executor (pixelcnn3.inc): any batch size, clusters of 16 CTAs per 4 / 8 samples
     launch_pixelcnn3(e, P, Q, audv, audh, label, noise, idx_out, logits_out, B, T0, Ttot, pre, logits_all, arena3, MB3, s, ctl, seeds,
-                     anchors, style, clip_ctl, clip_shape, code_bias);
+                     anchors, style, clip_ctl, clip_shape, code_bias, guide);
     return;
   }
   if (B > PIX_MB)
@@ -1827,6 +1901,7 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
   A.style = style; A.cls_w = P->d_cls; A.ncls = P->nclasses;
   A.clip_ctl = clip_ctl;
   A.clip_shape = clip_shape; A.code_bias = code_bias;
+  A.guide = guide;
   if (e->pixel_mode == 0) {
     // A/B switch: 0 = burst loads + scalar FFMA, 4 = pipelined loads + scalar FFMA, 5 (default) = pipelined loads + paired FMAs (fma2)
     static const int pipe = getenv("TS_PIX_PIPE") ? atoi(getenv("TS_PIX_PIPE")) : 5;
@@ -1901,22 +1976,33 @@ void pixel_destroy(ts_engine* e) {
 void pixelcnn_generate_act(ts_engine* e, const Act3& aud, const int64_t* label, const float* noise, int64_t* idx_out,
                            float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s, bool logits_all,
                            const SampleCtl* ctl, const int64_t* seeds, const int64_t* anchors, const float* style,
-                           const ts_clip_ctl* clip_ctl, const ts_clip_shape* clip_shape, const float* code_bias) {
+                           const ts_clip_ctl* clip_ctl, const ts_clip_shape* clip_shape, const float* code_bias,
+                           const float* guide) {
   if (!e->pix) fail(TS_ERR_NOT_LOADED, "pixelcnn weights not loaded");
-  // an anchored, styled, per-clip or shaped call always runs the WARP kernels; without controls at temperature 1, top_k 0
-  // (the default draw's bits)
+  // an anchored, styled, per-clip, shaped or guided call always runs the WARP kernels; without controls at temperature 1,
+  // top_k 0 (the default draw's bits)
   const SampleCtl dflt;
-  if ((anchors || style || clip_ctl || clip_shape || code_bias) && !ctl) ctl = &dflt;
-  // per-clip controls and shaping: host entries (validated by the caller) -> workspace, in stream order before the
-  // sampler reads them
-  ts_clip_ctl* dclip = clip_ctl ? e->ws.alloc<ts_clip_ctl>((size_t)B) : nullptr;
+  if ((anchors || style || clip_ctl || clip_shape || code_bias || guide) && !ctl) ctl = &dflt;
+  // per-clip (guided: per-pair) controls, shaping and scales: host entries (validated by the caller) -> workspace, in
+  // stream order before the sampler reads them
+  const size_t nd = guide ? (size_t)B / 2 : (size_t)B;
+  ts_clip_ctl* dclip = clip_ctl ? e->ws.alloc<ts_clip_ctl>(nd) : nullptr;
   if (dclip && !e->ws.sizing)
-    TS_CUDA(cudaMemcpyAsync(dclip, clip_ctl, (size_t)B * sizeof(ts_clip_ctl), cudaMemcpyHostToDevice, s));
-  ts_clip_shape* dshape = clip_shape ? e->ws.alloc<ts_clip_shape>((size_t)B) : nullptr;
+    TS_CUDA(cudaMemcpyAsync(dclip, clip_ctl, nd * sizeof(ts_clip_ctl), cudaMemcpyHostToDevice, s));
+  ts_clip_shape* dshape = clip_shape ? e->ws.alloc<ts_clip_shape>(nd) : nullptr;
   if (dshape && !e->ws.sizing)
-    TS_CUDA(cudaMemcpyAsync(dshape, clip_shape, (size_t)B * sizeof(ts_clip_shape), cudaMemcpyHostToDevice, s));
-  generate_chunk(e, aud, 0, label, noise, B, idx_out, logits_out, B, T, pre, T0, s, logits_all, ctl, seeds, anchors, style,
-                 dclip, dshape, code_bias);
+    TS_CUDA(cudaMemcpyAsync(dshape, clip_shape, nd * sizeof(ts_clip_shape), cudaMemcpyHostToDevice, s));
+  float* dguide = guide ? e->ws.alloc<float>(nd) : nullptr;
+  if (dguide && !e->ws.sizing) TS_CUDA(cudaMemcpyAsync(dguide, guide, nd * sizeof(float), cudaMemcpyHostToDevice, s));
+  // guided: pre_latents [P][T0][2] -> one copy per branch [2P][T0][2], so every pre read stays on the branch's own index
+  int64_t* dpre = guide && pre && T0 > 0 ? e->ws.alloc<int64_t>((size_t)B * T0 * 2) : nullptr;
+  if (dpre && !e->ws.sizing) {
+    const size_t row = (size_t)T0 * 2 * sizeof(int64_t);
+    for (int k = 0; k < 2; ++k)
+      TS_CUDA(cudaMemcpy2DAsync(reinterpret_cast<char*>(dpre) + k * row, 2 * row, pre, row, row, nd, cudaMemcpyDeviceToDevice, s));
+  }
+  generate_chunk(e, aud, 0, label, noise, B, idx_out, logits_out, B, T, dpre ? dpre : pre, T0, s, logits_all, ctl, seeds,
+                 anchors, style, dclip, dshape, code_bias, dguide);
 }
 
 void check_style(const ts_engine* e, const int64_t* label, const float* style, int ncls, const char* who) {
@@ -1985,6 +2071,14 @@ void check_clip_shape(const ts_clip_shape* clip_shape, int B, const char* who) {
     if (c.repetition_window < 1)
       fail(TS_ERR_INVALID, "%s: clip %d: repetition_window %d (must be >= 1)", who, b, c.repetition_window);
   }
+}
+
+void check_guidance(const float* guidance, int P, const char* who) {
+  if (!guidance) fail(TS_ERR_INVALID, "%s: guidance is NULL", who);
+  for (int p = 0; p < P; ++p)
+    if (!std::isfinite(guidance[p]) || !(guidance[p] >= 0.f && guidance[p] <= TS_GUIDANCE_MAX))
+      fail(TS_ERR_INVALID, "%s: pair %d: guidance %g (must be finite and in [0, %g])", who, p, (double)guidance[p],
+           (double)TS_GUIDANCE_MAX);
 }
 
 SampleCtl sample_ctl_of(const ts_sample_ctl* c) {
@@ -2128,7 +2222,8 @@ static void pixelcnn_generate_call(ts_engine* e, const float* aud, const int64_t
                                    float* logits_out, int B, int T, const int64_t* pre_latents, int T0, void* stream,
                                    const SampleCtl* ctl, const int64_t* seeds = nullptr, const int64_t* anchors = nullptr,
                                    const float* style = nullptr, const ts_clip_ctl* clip_ctl = nullptr,
-                                   const ts_clip_shape* clip_shape = nullptr, const float* code_bias = nullptr) {
+                                   const ts_clip_shape* clip_shape = nullptr, const float* code_bias = nullptr,
+                                   const float* guide = nullptr) {
   check_pix(e, B, T);
   if (T0 < 0 || (T0 > 0 && !pre_latents)) fail(TS_ERR_INVALID, "pixelcnn: T0=%d without pre_latents", T0);
   if (ctl && !clip_ctl) check_sample_ctl(*ctl, noise, seeds);
@@ -2137,7 +2232,7 @@ static void pixelcnn_generate_call(ts_engine* e, const float* aud, const int64_t
     Act3 a = new_act(e, B, T0 + T, 256, 0, s);
     nct_to_act(e, aud, 256, a, s);
     pixelcnn_generate_act(e, a, label, noise, idx_out, logits_out, B, T, pre_latents, T0, s, false, ctl, seeds, anchors, style,
-                          clip_ctl, clip_shape, code_bias);
+                          clip_ctl, clip_shape, code_bias, guide);
   };
   e->ws.begin_sizing(); body();
   size_t need = e->ws.need;
@@ -2277,6 +2372,25 @@ extern "C" int ts_pixelcnn_sample_shaped(ts_engine* e, const float* aud, const i
   const SampleCtl c = shaped_ctl(ctl, clip_ctl, B, noise, seeds, "ts_pixelcnn_sample_shaped");
   pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, &c, seeds, anchors, style,
                          clip_ctl, clip_shape, code_bias);
+  TS_API_END(e)
+}
+
+// P pairs = 2P branches: aud / label / style / idx_out / logits_out / logp / kept per branch, every draw input per pair.
+// guidance [P] (host): checked here and copied to the workspace on the call's stream.
+extern "C" int ts_pixelcnn_sample_guided(ts_engine* e, const float* aud, const int64_t* label, const float* style, int ncls,
+                                         const float* noise, const int64_t* seeds, const int64_t* anchors, int64_t* idx_out,
+                                         float* logits_out, int P, int T, const int64_t* pre_latents, int T0,
+                                         const ts_sample_ctl* ctl, const ts_clip_ctl* clip_ctl, const ts_clip_shape* clip_shape,
+                                         const float* code_bias, const float* guidance, void* stream) {
+  TS_API_BEGIN(e)
+  if (P < 1 || P > INT_MAX / 2) fail(TS_ERR_INVALID, "ts_pixelcnn_sample_guided: P=%d pairs", P);
+  check_pix(e, 2 * P, T);
+  check_style(e, label, style, ncls, "ts_pixelcnn_sample_guided");
+  check_guidance(guidance, P, "ts_pixelcnn_sample_guided");
+  if (clip_shape) check_clip_shape(clip_shape, P, "ts_pixelcnn_sample_guided");
+  const SampleCtl c = shaped_ctl(ctl, clip_ctl, P, noise, seeds, "ts_pixelcnn_sample_guided");
+  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, 2 * P, T, pre_latents, T0, stream, &c, seeds, anchors,
+                         style, clip_ctl, clip_shape, code_bias, guidance);
   TS_API_END(e)
 }
 

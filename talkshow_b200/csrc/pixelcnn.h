@@ -95,12 +95,15 @@ SampleCtl sample_ctl_of(const ts_sample_ctl* c);
 // ts_pixelcnn_sample_clips, copied to the workspace on s; each clip draws with its entry in place of ctl's four controls.
 // clip_shape [B] (HOST, validated with check_clip_shape) and code_bias [B,2,2048] (device): the logit shaping of
 // ts_pixelcnn_sample_shaped, likewise on the WARP kernels (clip_shape copied to the workspace on s).
+// guide [B / 2] (HOST, validated with check_guidance): the scales of ts_pixelcnn_sample_guided, copied to the workspace on
+// s.  B is then the branch count 2P: aud, label, style, idx_out and logits_out are per branch; noise [2T][P][2048], seeds,
+// anchors, pre, clip_ctl, clip_shape and code_bias are per pair (pre is copied once per branch into the workspace).
 void pixelcnn_generate_act(ts_engine* e, const Act3& aud, const int64_t* label, const float* noise, int64_t* idx_out,
                            float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s,
                            bool logits_all = false, const SampleCtl* ctl = nullptr, const int64_t* seeds = nullptr,
                            const int64_t* anchors = nullptr, const float* style = nullptr,
                            const ts_clip_ctl* clip_ctl = nullptr, const ts_clip_shape* clip_shape = nullptr,
-                           const float* code_bias = nullptr);
+                           const float* code_bias = nullptr, const float* guide = nullptr);
 // The class terms of gate channel q (tanh half) and D + q (sigmoid half) under one row's speaker weights w[0..ncls)
 // (ts_pixelcnn_sample_styled): acc = w0 E[0][ch], then acc + w_s E[s][ch] for s = 1 .. ncls-1, every product and sum
 // rounded to fp32 without contraction.  tab: one layer's class_cond_embedding [ncls][2D]; w null (a padding sample of the
@@ -131,12 +134,17 @@ void check_clip_ctl(const ts_clip_ctl* clip_ctl, int B, const float* noise, cons
 // The per-clip shaping of ts_pixelcnn_sample_shaped (TS_ERR_INVALID, naming the clip): a finite repetition_penalty >= 1
 // and a repetition_window >= 1.  clip_shape: B host entries.
 void check_clip_shape(const ts_clip_shape* clip_shape, int B, const char* who);
+// The scales of ts_pixelcnn_sample_guided (TS_ERR_INVALID, naming the pair): P host values, each finite and in
+// [0, TS_GUIDANCE_MAX]; NULL is refused.
+void check_guidance(const float* guidance, int P, const char* who);
 // The controls of a shaped call: with clip_ctl, check_clip_ctl and ctl's logp_out / kept_out; else ctl's controls (the
 // default draw when ctl is NULL), checked with check_sample_ctl and check_anchored_source.
 SampleCtl shaped_ctl(const ts_sample_ctl* ctl, const ts_clip_ctl* clip_ctl, int B, const float* noise, const int64_t* seeds,
                      const char* who);
 // idx [B,T,2] -> idx_c [2][B][T]; optionally copies idx to codes_out
 void split_codes(ts_engine* e, const int64_t* idx, int64_t* idx_c, int B, int T, int64_t* codes_out, cudaStream_t s);
+// A guided call's idx [2P,T,2] -> idx_c [2][P][T] of the conditional branches (rows 2p); optionally copies idx to codes_out
+void split_guided_codes(ts_engine* e, const int64_t* idx, int64_t* idx_c, int P, int T, int64_t* codes_out, cudaStream_t s);
 void pixel_destroy(ts_engine* e);
 // weights of ts_pixelcnn_score packed for its GEMMs (pixelcnn_tf.cu); nullptr on a host-only engine
 void* tf_build(ts_engine* e, const Ckpt& ck, int L, int D, int ncls);

@@ -230,6 +230,69 @@ def shaping_kwargs(repetition_penalty=1.0, repetition_window=8, code_bias=None, 
     return dict(repetition_penalty=repetition_penalty, repetition_window=repetition_window, code_bias=code_bias)
 
 
+GUIDANCE_MAX = 100.0   # largest guidance scale (include/talkshow_b200.h TS_GUIDANCE_MAX)
+GUIDE_PAIRS = PIX_TILE // 2   # pairs per guided launch: two branches each, one 64-sample tile
+
+
+def check_guidance(guidance, B):
+    """Guidance scales of a guided call as a float32 host array [B]: a scalar, applied to every clip, or one value per clip
+    (a length-B sequence, 1-D numpy array or 1-D tensor).  Each value must be a number whose fp32 value is finite and in
+    [0, 100] (1 = no guidance).  Anything else raises ValueError naming the clip."""
+    vals = _clip_values("guidance", guidance, B) if _is_per_clip(guidance) else [guidance] * B
+    out = np.zeros(B, np.float32)
+    for b, w in enumerate(vals):
+        try:
+            if isinstance(w, bool):
+                raise TypeError
+            with np.errstate(over="ignore"):
+                w32 = np.float32(float(w))
+        except (TypeError, ValueError):
+            raise ValueError("guidance: clip %d: must be a number, got %r" % (b, w)) from None
+        if not (math.isfinite(w32) and 0.0 <= w32 <= GUIDANCE_MAX):
+            raise ValueError("guidance: clip %d: must be finite and in [0, %g] (1 = no guidance), got %r" % (b, GUIDANCE_MAX, w))
+        out[b] = w32
+    return out
+
+
+def guide_kwargs(guidance=None, guide_mfcc=None, guide_label=None, guide_style=None, keep_logp=False, engine=None, B=None,
+                 M=None):
+    """The guidance keywords a caller forwards to ``Engine.body_generate``: none without ``guidance`` (the call then
+    forwards what it forwarded before; a negative conditioning without guidance raises ValueError).  ``guide_mfcc`` may be
+    the string "silence": ``engine.silence_mfcc(M, B)``.  ``keep_logp`` asks for the negative branches' log p too."""
+    if guidance is None:
+        if guide_mfcc is not None or guide_label is not None or guide_style is not None:
+            raise ValueError("a negative conditioning (guide_mfcc / guide_id / guide_style) needs guidance")
+        return {}
+    if isinstance(guide_mfcc, str):
+        if guide_mfcc != "silence":
+            raise ValueError("guide_mfcc: the only named conditioning is \"silence\", got %r" % (guide_mfcc,))
+        guide_mfcc = engine.silence_mfcc(M, B)
+    return dict(guidance=guidance, guide_mfcc=guide_mfcc, guide_label=guide_label, guide_style=guide_style,
+                want_guide_logp=bool(keep_logp))
+
+
+def _same_input(a, b):
+    """Whether a negative-conditioning field repeats the clip's own, decided without a device synchronisation: the same
+    object, equal host values (a one-element label broadcast), or a device tensor viewing the same memory.  Two device
+    tensors with equal values in different memory count as different."""
+    if a is b:
+        return True
+    if torch.is_tensor(a) and a.is_cuda or torch.is_tensor(b) and b.is_cuda:
+        return (torch.is_tensor(a) and torch.is_tensor(b) and a.device == b.device and a.dtype == b.dtype
+                and a.shape == b.shape and a.stride() == b.stride() and a.data_ptr() == b.data_ptr())
+    a, b = torch.as_tensor(np.asarray(a)), torch.as_tensor(np.asarray(b))
+    try:
+        a, b = torch.broadcast_tensors(a, b)
+    except RuntimeError:
+        return False
+    return bool(torch.equal(a, b.to(a.dtype)))
+
+
+def _interleave(x, g):
+    """Rows b of x and g as rows 2b and 2b + 1 of one tensor (the branches of a guided call)."""
+    return torch.stack([x, g], 1).reshape((2 * x.shape[0],) + tuple(x.shape[1:])).contiguous()
+
+
 def sampled(temperature):
     """True when a call with this (validated) temperature draws noise: temperature > 0, for some clip when per clip."""
     if _is_per_clip(temperature):
@@ -506,6 +569,21 @@ class Engine:
         self._check(self.L.ts_mfcc(self.h, _lib.ptr(wave), _lib.ptr(out), B, N, int(sr), self._s()), "ts_mfcc")
         return out
 
+    def silence_mfcc(self, M, B=1):
+        """The MFCC [B,64,M] of a silent clip of M frames: ``mfcc`` (the device front end) on a zero waveform at 22 kHz
+        whose length gives exactly M frames.  A negative conditioning for audio guidance (``body_generate``)."""
+        M = int(M)
+        if M < 1:
+            raise ValueError("silence_mfcc: M = %d frames" % M)
+        n = max(1, (M - 1) * 734)
+        while self.L.ts_mfcc_frames(n, 22000) < M:
+            n += 1
+        while n > 1 and self.L.ts_mfcc_frames(n - 1, 22000) >= M:
+            n -= 1
+        if self.L.ts_mfcc_frames(n, 22000) != M:
+            raise ValueError("silence_mfcc: no waveform length gives %d frames" % M)
+        return self.mfcc(torch.zeros(1, n), 22000).repeat(B, 1, 1)
+
     def audio_encode(self, mfcc):
         """AudioEncoder.forward: [B,64,M] -> [B,256,T]."""
         mfcc = self._dev(mfcc, torch.float32)
@@ -532,7 +610,8 @@ class Engine:
 
     def pixelcnn_generate(self, aud, label, noise, T=None, pre_latents=None, want_logits=False, temperature=1.0, top_k=0,
                           want_logp=False, top_p=1.0, min_p=0.0, want_kept=False, seeds=None, anchors=None, style=None,
-                          repetition_penalty=1.0, repetition_window=8, code_bias=None):
+                          repetition_penalty=1.0, repetition_window=8, code_bias=None, guidance=None, guide_aud=None,
+                          guide_label=None, guide_style=None, want_guide_logp=False):
         """GatedPixelCNN.generate: aud [B,256,T0+T], label [B], noise [2T,B,2048] -> codes [B,T,2]
         (+ logits [2T,B,2048]).  Batches above the 64-sample tile are chunked here.
 
@@ -571,7 +650,26 @@ class Engine:
         column in the clip's previous ``repetition_window`` rows (prefix rows and pinned draws included); ``code_bias``
         (``check_code_bias``: [2,2048] or [B,2,2048], -inf bans a code) is then added.  The controls act on the shaped
         logits; logp stays that of the raw prior.  The penalty and window take a scalar or one value per clip
-        (``check_clip_shape``).  Without a bias and with theta 1 everywhere the call forwards what it forwarded before."""
+        (``check_clip_shape``).  Without a bias and with theta 1 everywhere the call forwards what it forwarded before.
+
+        Guided sampling (ts_pixelcnn_sample_guided; rule in include/talkshow_b200.h): ``guidance`` w (``check_guidance``:
+        scalar or per clip, in [0, 100], 1 = none) draws every code from g = l_c + (w - 1) (l_c - l_u), l_c the clip's
+        logits and l_u those under a negative conditioning: ``guide_aud`` [B,256,T0+T], ``guide_label`` [B] and / or
+        ``guide_style`` (as ``style``).  A field not given copies the clip's own; at least one must be given and differ.
+        The negative branch is fed the guided codes, so both branches follow the same motion.  The check that the negative
+        differs reads no device data: a device tensor counts as the clip's own only when it is the same memory.  Every draw input stays per
+        clip; logp is the clip's conditional log p; ``want_guide_logp`` appends the negative branch's log p [B,T,2];
+        ``want_logits`` gives the raw logits of both branches, [2T,2B,2048] with clip b's in column 2b.  Each
+        launch holds 32 clips (64 branches).  Without ``guidance`` the call forwards what it forwarded before."""
+        if guidance is not None:
+            return self._guided("pixel", aud, label, noise, T=T, pre_latents=pre_latents, want_logits=want_logits,
+                                temperature=temperature, top_k=top_k, want_logp=want_logp, top_p=top_p, min_p=min_p,
+                                want_kept=want_kept, seeds=seeds, anchors=anchors, style=style,
+                                repetition_penalty=repetition_penalty, repetition_window=repetition_window,
+                                code_bias=code_bias, guidance=guidance, guide_cond=guide_aud, guide_label=guide_label,
+                                guide_style=guide_style, want_guide_logp=want_guide_logp)
+        if guide_aud is not None or guide_label is not None or guide_style is not None or want_guide_logp:
+            raise ValueError("pixelcnn_generate: guide_aud / guide_label / guide_style / want_guide_logp need guidance")
         clip = None
         if per_clip(temperature, top_k, top_p, min_p):
             clip = check_clip_controls(temperature, top_k, top_p, min_p, aud.shape[0])
@@ -798,7 +896,8 @@ class Engine:
 
     def body_generate(self, mfcc, label, noise, want_codes=True, temperature=1.0, top_k=0, want_logp=False, top_p=1.0,
                       min_p=0.0, want_kept=False, seeds=None, anchors=None, style=None, repetition_penalty=1.0,
-                      repetition_window=8, code_bias=None):
+                      repetition_window=8, code_bias=None, guidance=None, guide_mfcc=None, guide_label=None,
+                      guide_style=None, want_guide_logp=False):
         """fused s2g_body_pixel core: mfcc [B,64,M] -> (codes [B,T,2], poses [B,4T,C]), C = 129 (258 for 6-D).
         Sampling controls as in ``pixelcnn_generate`` (ts_body_sample, ts_body_sample_ctl); ``want_logp`` appends logp
         [B,T,2], ``want_kept`` then kept [B,T,2] int32.  ``seeds`` [B] in place of ``noise``: seeded sampling
@@ -807,7 +906,19 @@ class Engine:
         ``style`` [B,T,ncls] or [B,ncls]: a speaker schedule as in ``pixelcnn_generate`` (ts_body_sample_styled; label
         may then be None).  Per-clip ``temperature`` / ``top_k`` / ``top_p`` / ``min_p`` as in ``pixelcnn_generate``
         (ts_body_sample_clips); each clip's poses decode its own codes.  ``repetition_penalty`` / ``repetition_window`` /
-        ``code_bias``: logit shaping as in ``pixelcnn_generate`` (ts_body_sample_shaped)."""
+        ``code_bias``: logit shaping as in ``pixelcnn_generate`` (ts_body_sample_shaped).  ``guidance`` with ``guide_mfcc``
+        [B,64,M] / ``guide_label`` / ``guide_style``: guided sampling as in ``pixelcnn_generate`` (ts_body_sample_guided);
+        codes and poses are the clips' (the negative branches are not decoded), ``want_guide_logp`` appends the negative
+        branches' log p [B,T,2]."""
+        if guidance is not None:
+            return self._guided("body", mfcc, label, noise, want_codes=want_codes, temperature=temperature, top_k=top_k,
+                                want_logp=want_logp, top_p=top_p, min_p=min_p, want_kept=want_kept, seeds=seeds,
+                                anchors=anchors, style=style, repetition_penalty=repetition_penalty,
+                                repetition_window=repetition_window, code_bias=code_bias, guidance=guidance,
+                                guide_cond=guide_mfcc, guide_label=guide_label, guide_style=guide_style,
+                                want_guide_logp=want_guide_logp)
+        if guide_mfcc is not None or guide_label is not None or guide_style is not None or want_guide_logp:
+            raise ValueError("body_generate: guide_mfcc / guide_label / guide_style / want_guide_logp need guidance")
         clip = None
         if per_clip(temperature, top_k, top_p, min_p):
             clip = check_clip_controls(temperature, top_k, top_p, min_p, mfcc.shape[0])
@@ -894,6 +1005,109 @@ class Engine:
             else:
                 self._check(self.L.ts_body_generate(*args, self._s()), "ts_body_generate")
         return (codes, poses) + ((logp,) if want_logp else ()) + ((kept,) if want_kept else ())
+
+    def _guided(self, kind, cond, label, noise, T=None, pre_latents=None, want_logits=False, want_codes=True,
+                temperature=1.0, top_k=0, want_logp=False, top_p=1.0, min_p=0.0, want_kept=False, seeds=None, anchors=None,
+                style=None, repetition_penalty=1.0, repetition_window=8, code_bias=None, guidance=None, guide_cond=None,
+                guide_label=None, guide_style=None, want_guide_logp=False):
+        """The guided calls of ``pixelcnn_generate`` (kind "pixel", cond = aud) and ``body_generate`` (kind "body", cond =
+        mfcc): B clips -> 2B interleaved branches (2b the clip, 2b + 1 its negative conditioning), every draw input per
+        clip, GUIDE_PAIRS clips per launch."""
+        who = "pixelcnn_generate" if kind == "pixel" else "body_generate"
+        B = cond.shape[0]
+        w = check_guidance(guidance, B)
+        if guide_cond is None and guide_label is None and guide_style is None:
+            raise ValueError("%s: guidance needs a negative conditioning (guide_%s, guide_label or guide_style)"
+                             % (who, "aud" if kind == "pixel" else "mfcc"))
+        clip = None
+        if per_clip(temperature, top_k, top_p, min_p):
+            clip = check_clip_controls(temperature, top_k, top_p, min_p, B)
+            _clip_source(clip, noise, seeds)
+        else:
+            _controlled(temperature, top_k, noise, want_logp, top_p, min_p, want_kept, seeds)
+        shape = check_clip_shape(repetition_penalty, repetition_window, B)
+        penalised = bool((shape["repetition_penalty"] != 1.0).any())
+        bias = None if code_bias is None else self._dev(check_code_bias(code_bias, B), torch.float32)
+        # the negative must differ from the clip in some field (checked on the inputs as given: no synchronisation)
+        if guide_label is not None:
+            same_class = label is not None and style is None and guide_style is None and _same_input(label, guide_label)
+        elif guide_style is not None:
+            same_class = style is not None and _same_input(style, guide_style)
+        else:
+            same_class = True
+        if same_class and (guide_cond is None or _same_input(cond, guide_cond)):
+            raise ValueError("%s: the negative conditioning equals the clips' own: guidance would change nothing" % who)
+        cond = self._dev(cond, torch.float32)
+        gcond = cond if guide_cond is None else self._dev(guide_cond, torch.float32)
+        if tuple(gcond.shape) != tuple(cond.shape):
+            raise ValueError("%s: the negative conditioning has shape %s, the clips %s"
+                             % (who, tuple(gcond.shape), tuple(cond.shape)))
+        if label is None and style is None:
+            raise ValueError("%s: label is required without style" % who)
+        T0 = 0 if pre_latents is None else pre_latents.shape[1]
+        if kind == "pixel":
+            T = cond.shape[2] - T0 if T is None else T
+        else:
+            T = self.latent_rows(cond.shape[2])
+        ncls = self.pixelcnn_ncls
+
+        def labels(v):
+            v = self._dev(v if torch.is_tensor(v) else torch.as_tensor(v), torch.int64).reshape(-1)
+            return v.expand(B).contiguous() if v.numel() == 1 and B > 1 else v
+
+        def one_hot(v):   # a label as its one-hot schedule, which draws what the label draws (ts_pixelcnn_sample_styled)
+            return torch.nn.functional.one_hot(v.clamp(0, ncls - 1), ncls).to(torch.float32)
+
+        label = None if label is None else labels(label)
+        glabel = None if guide_label is None else labels(guide_label)
+        style = None if style is None else self._dev(check_style(style, B, T0 + T, ncls), torch.float32)
+        gstyle = None if guide_style is None else self._dev(check_style(guide_style, B, T0 + T, ncls), torch.float32)
+        if style is None and gstyle is None:   # labels on both branches
+            label2, style2 = _interleave(label, label if glabel is None else glabel), None
+        else:                                  # a schedule on either side: both branches as schedules
+            cs = style if style is not None else one_hot(label)[:, None, :].expand(B, T0 + T, ncls)
+            gs = gstyle if gstyle is not None else (one_hot(glabel)[:, None, :].expand(B, T0 + T, ncls)
+                                                    if glabel is not None else cs)
+            label2, style2 = None, _interleave(cs, gs)
+        cond2 = _interleave(cond, gcond)
+        noise = None if noise is None else self._dev(noise, torch.float32)
+        seeds = None if seeds is None else self._dev(check_seeds(seeds, B), torch.int64)
+        anchors = None if anchors is None else self._dev(check_anchors(anchors, B, T), torch.int64)
+        pre = None if pre_latents is None else self._dev(pre_latents, torch.int64)
+        idx = torch.empty(2 * B, T, 2, dtype=torch.int64, device=self.device) if (kind == "pixel" or want_codes) else None
+        logits = torch.empty(2 * T, 2 * B, 2048, device=self.device) if want_logits else None
+        lp = torch.empty(2 * B, T, 2, device=self.device) if (want_logp or want_guide_logp) else None
+        kept = torch.empty(2 * B, T, 2, dtype=torch.int32, device=self.device) if want_kept else None
+        poses = torch.empty(B, 4 * T, self.vq_dim(0) + self.vq_dim(1), device=self.device) if kind == "body" else None
+        sl = lambda t, a, b: None if t is None else t[a:b].contiguous()
+        for b0 in range(0, B, GUIDE_PAIRS):
+            b1 = min(B, b0 + GUIDE_PAIRS)
+            nb, r0, r1 = b1 - b0, 2 * b0, 2 * b1
+            nz = noise if (noise is None or nb == B) else noise[:, b0:b1].contiguous()
+            lz = None if logits is None else (logits if nb == B else torch.empty(2 * T, 2 * nb, 2048, device=self.device))
+            c = (_ctl_struct(1.0, 0, 1.0, 0.0, sl(lp, r0, r1), sl(kept, r0, r1)) if clip is not None
+                 else _ctl_struct(temperature, top_k, top_p, min_p, sl(lp, r0, r1), sl(kept, r0, r1)))
+            head = (self.h, _lib.ptr(cond2[r0:r1]), _lib.ptr(sl(label2, r0, r1)), _lib.ptr(sl(style2, r0, r1)), ncls,
+                    _lib.ptr(nz), _lib.ptr(sl(seeds, b0, b1)), _lib.ptr(sl(anchors, b0, b1)))
+            tail = (C.byref(c), None if clip is None else clip[b0:b1].ctypes.data,
+                    shape[b0:b1].ctypes.data if penalised else None, _lib.ptr(sl(bias, b0, b1)), w[b0:b1].ctypes.data,
+                    self._s())
+            if kind == "pixel":
+                self._check(self.L.ts_pixelcnn_sample_guided(*head, _lib.ptr(idx[r0:r1]), _lib.ptr(lz), nb, T,
+                                                             _lib.ptr(sl(pre, b0, b1)), T0, *tail), "ts_pixelcnn_sample_guided")
+            else:
+                self._check(self.L.ts_body_sample_guided(*head, _lib.ptr(None if idx is None else idx[r0:r1]),
+                                                         _lib.ptr(poses[b0:b1]), nb, cond.shape[2], *tail),
+                            "ts_body_sample_guided")
+            if lz is not None and nb != B:
+                logits[:, r0:r1] = lz
+        codes = None if idx is None else idx[0::2].contiguous()
+        extra = (((lp[0::2].contiguous(),) if want_logp else ()) + ((kept[0::2].contiguous(),) if want_kept else ())
+                 + ((lp[1::2].contiguous(),) if want_guide_logp else ()))
+        if kind == "body":
+            return (codes, poses) + extra
+        out = (codes,) + ((logits,) if want_logits else ()) + extra
+        return out if len(out) > 1 else codes
 
     # -- the single collective of the path, inside the library (ts_allgather over a dlopen'ed NCCL) ----------------
     @staticmethod

@@ -10,7 +10,7 @@ import torch
 
 from ..data_utils.lower_body import c_index_3d, c_index_6d
 from ..data_utils.utils import get_mfcc_sepa, get_mfcc_ta, load_wav
-from ..engine import (check_clip_controls, check_sample_controls, check_style, per_clip, resolve_clip_seeds, sample_controls,
+from ..engine import (check_clip_controls, guide_kwargs, check_sample_controls, check_style, per_clip, resolve_clip_seeds, sample_controls,
                       sampled, shaping_kwargs)
 from .base import draw_sampler_noise, resolve_device, shared_engine, strip_module
 
@@ -109,10 +109,21 @@ class TrainWrapper:
 
     def infer_on_audio(self, aud_fn, initial_pose=None, norm_stats=None, exp=None, var=None, w_pre=False, rand=None,
                        continuity=False, id=None, fps=15, sr=22000, B=1, am=None, am_sr=None, frame=0, **kwargs):
-        """(aud_fn) -> generated motion, numpy (B, F, 129).  Reference: :232-289."""
+        """(aud_fn) -> generated motion, numpy (B, F, 129).  Reference: :232-289.  Guidance as in ``generate``
+        (``guidance``, ``guide_id``, ``guide_style``); ``guide_audio`` is "silence" or (M, 64) features like an array
+        ``aud_fn``.  Not with ``continuity``."""
         assert self.args.infer, "train mode"
         ctl = {k: kwargs[k] for k in ("temperature", "top_k", "keep_logp", "top_p", "min_p", "clip_seeds", "repetition_penalty",
                                       "repetition_window", "code_bias") if k in kwargs}
+        if kwargs.get("guidance") is not None:
+            if continuity:
+                raise ValueError("infer_on_audio: guidance is not supported with continuity=True (the clip is cut into "
+                                 "two chunks); guide each chunk through infer()")
+            ga = kwargs.get("guide_audio")
+            if ga is not None and not isinstance(ga, str):
+                ga = torch.from_numpy(np.ascontiguousarray(np.asarray(ga, dtype=np.float32).T))[None].repeat(B, 1, 1)
+            ctl.update(guidance=kwargs["guidance"], guide_mfcc=ga, guide_id=kwargs.get("guide_id"),
+                       guide_style=kwargs.get("guide_style"))
         if kwargs.get("noise_fn") is not None and kwargs.get("clip_seeds") is not None:
             raise ValueError("infer_on_audio: noise_fn and clip_seeds are two noise sources; give one")
         if kwargs.get("anchors") is not None:
@@ -137,7 +148,8 @@ class TrainWrapper:
         return self.generate(mfcc, label, noise_fn=kwargs.get("noise_fn"), **ctl).cpu().numpy()
 
     def generate(self, aud, id, frame_num=0, noise_fn=None, temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0,
-                 clip_seeds=None, anchors=None, style=None, repetition_penalty=1.0, repetition_window=8, code_bias=None):
+                 clip_seeds=None, anchors=None, style=None, repetition_penalty=1.0, repetition_window=8, code_bias=None,
+                 guidance=None, guide_mfcc=None, guide_id=None, guide_style=None):
         """tensor API (:306-326): aud [B,64,M] features, id [B] -> torch (B, F, 129) on the device.
         (The reference's version passes decode()'s tuple to torch.cat and raises; this returns the
         tensor its infer_on_audio builds.)
@@ -168,12 +180,20 @@ class TrainWrapper:
         Logit shaping (Engine.pixelcnn_generate): ``repetition_penalty`` (>= 1, 1 = off; scalar or per clip) penalises the
         codes the clip drew at the same column in its last ``repetition_window`` latent rows (8 rows, about 1 s), which
         breaks the loops greedy or cold sampling falls into; ``code_bias`` [2,2048] or [B,2,2048] is added to the logits
-        (column 0 body codes, column 1 hand codes; -inf never draws the code)."""
+        (column 0 body codes, column 1 hand codes; -inf never draws the code).
+
+        Guidance (Engine.body_generate): ``guidance`` w (scalar or per clip, in [0, 100]; 1 = none) pushes every draw
+        away from a negative conditioning: ``guide_mfcc`` [B,64,M] or "silence" (audio guidance: gestures that follow the
+        speech more closely), ``guide_id`` [B] (another speaker) and / or ``guide_style`` (e.g. a uniform blend).  Fields
+        not given copy the clip's own.  The prior was trained without condition dropout, so this is contrastive guidance
+        against the chosen conditioning.  With ``keep_logp`` the negative branches' log p is kept as
+        self.last_guide_logp."""
         mfcc = aud.to(torch.float32)
         B, _, M = mfcc.shape
         T = self.engine.latent_rows(M)
         seeds = self._seeds(clip_seeds, B, noise_fn)
         shaping = shaping_kwargs(repetition_penalty, repetition_window, code_bias, B)
+        guide = guide_kwargs(guidance, guide_mfcc, guide_id, guide_style, keep_logp, self.engine, B, M)
         noise = self._draw_noise(T, B, noise_fn, temperature, top_k, top_p, min_p, seeds)
         ctl = sample_controls(temperature, top_k, keep_logp, top_p, min_p)
         ctl.update(shaping)
@@ -183,10 +203,12 @@ class TrainWrapper:
             ctl["anchors"] = anchors
         if style is not None:
             ctl["style"] = style
+        ctl.update(guide)
         out = self.engine.body_generate(mfcc, id.to(torch.int64), noise, **ctl)
         self.last_codes, poses = out[0], out[1]
         self.last_logp = out[2] if keep_logp else None
         self.last_kept = out[3] if ctl.get("want_kept") else None
+        self.last_guide_logp = out[-1] if guide and keep_logp else None
         return poses
 
     def _draw_noise(self, T, B, noise_fn, temperature, top_k, top_p=1.0, min_p=0.0, seeds=None):
@@ -209,7 +231,8 @@ class TrainWrapper:
 
     def infer(self, aud_feat, frame, id, B, pre_latents=None, pre_audio=None, pre_pose=None, noise_fn=None,
               temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None, anchors=None, style=None,
-              repetition_penalty=1.0, repetition_window=8, code_bias=None):
+              repetition_penalty=1.0, repetition_window=8, code_bias=None, guidance=None, guide_mfcc=None, guide_id=None,
+              guide_style=None, guide_pre_audio=None):
         """The reference's inner call (:291-304): aud_feat [B,M,64] (time-major features of ONE chunk) ->
         (latents [B,T,2], audio [B,256,T,2], body [B,39,4T], hand [B,90,4T]).  ``pre_latents`` / ``pre_audio`` (the first
         two results of the previous chunk's call) condition the sampler on that chunk (GatedPixelCNN.generate :158-165);
@@ -221,12 +244,19 @@ class TrainWrapper:
         ``anchors`` [B,T,2] cover this chunk's T rows (as in ``generate``); with ``pre_latents`` they pin rows after the
         prefix.  ``style`` [B,T0+T,4] (or [B,4]) as in ``generate``, its rows covering the prefix and the chunk.  Per-clip
         controls and logit shaping as in ``generate``; with ``pre_latents`` the repetition window reaches back into the
-        prefix's codes."""
+        prefix's codes.  Guidance as in ``generate``, with ``guide_mfcc`` [B,M,64] (time-major like ``aud_feat``) or
+        "silence"; with ``pre_latents`` the negative branch's prefix audio is ``guide_pre_audio`` (default: the clip's
+        ``pre_audio``), and both branches are fed the prefix codes."""
         a = self.engine.audio_encode(aud_feat.transpose(1, 2).contiguous())            # [B,256,T]
         T = a.shape[2]
         label = id.reshape(-1)
         seeds = self._seeds(clip_seeds, B, noise_fn)
         shaping = shaping_kwargs(repetition_penalty, repetition_window, code_bias, B)
+        if isinstance(guide_mfcc, str):   # "silence" (guide_kwargs refuses any other name): [B,64,M] from the front end
+            gmc = guide_mfcc if guide_mfcc != "silence" else self.engine.silence_mfcc(aud_feat.shape[1], B)
+        else:                             # time-major [B,M,64] like aud_feat -> [B,64,M]
+            gmc = None if guide_mfcc is None else guide_mfcc.transpose(1, 2).contiguous()
+        guide = guide_kwargs(guidance, gmc, guide_id, guide_style, keep_logp, self.engine, B, aud_feat.shape[1])
         noise = self._draw_noise(T, B, noise_fn, temperature, top_k, top_p, min_p, seeds)
         ctl = sample_controls(temperature, top_k, keep_logp, top_p, min_p)
         ctl.update(shaping)
@@ -236,15 +266,25 @@ class TrainWrapper:
             ctl["anchors"] = anchors
         if style is not None:
             ctl["style"] = style
+        if guide:
+            gm = guide.pop("guide_mfcc")                   # [B,64,M] or None
+            ga = None if gm is None else self.engine.audio_encode(gm)
+            if pre_latents is not None:
+                gpa = pre_audio if guide_pre_audio is None else guide_pre_audio
+                gpa = gpa[..., 0] if gpa.dim() == 4 else gpa
+                ga = torch.cat([gpa.to(a.device), a if ga is None else ga], 2)
+            guide["guide_aud"] = ga
+            ctl.update(guide)
         if pre_latents is None:
             out = self.engine.pixelcnn_generate(a, label, noise, **ctl)
         else:
             pa = pre_audio[..., 0] if pre_audio.dim() == 4 else pre_audio              # [B,256,T0]
             out = self.engine.pixelcnn_generate(torch.cat([pa.to(a.device), a], 2), label, noise, T=T,
                                                 pre_latents=pre_latents, **ctl)
-        latents = out[0] if keep_logp else out
+        latents = out[0] if (keep_logp or guide) and isinstance(out, tuple) else out
         self.last_logp = out[1] if keep_logp else None
         self.last_kept = out[2] if ctl.get("want_kept") else None
+        self.last_guide_logp = out[-1] if guide and keep_logp else None
         body = self.engine.vq_decode(0, latents[..., 0].contiguous())
         hand = self.engine.vq_decode(1, latents[..., 1].contiguous())
         return latents, a.unsqueeze(-1).repeat(1, 1, 1, 2), body, hand

@@ -10,8 +10,8 @@ from __future__ import annotations
 
 import torch
 
-from .engine import (Engine, check_anchors, check_clip_controls, check_clip_shape, check_code_bias, check_style, per_clip,
-                     resolve_clip_seeds, sample_controls, sampled, shaping_kwargs)
+from .engine import (Engine, check_anchors, check_clip_controls, check_clip_shape, check_code_bias, check_guidance, check_style,
+                     guide_kwargs, per_clip, resolve_clip_seeds, sample_controls, sampled, shaping_kwargs)
 from .nets.base import draw_sampler_noise
 
 
@@ -80,7 +80,8 @@ class WholeBody:
 
     def generate(self, mfcc, wave, label, noise=None, stand=False, per_step_noise=True, temperature=1.0, top_k=0,
                  keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None, anchors=None, keep_codes=False, style=None,
-                 repetition_penalty=1.0, repetition_window=8, code_bias=None):
+                 repetition_penalty=1.0, repetition_window=8, code_bias=None, guidance=None, guide_mfcc=None, guide_label=None,
+                 guide_style=None):
         """mfcc [B,64,M], wave [B,N] (16 kHz), label [B] on the device -> poses [B,F,265] (device).
         F = N*30//16000 face frames; the body (4*T frames) is padded/truncated to F like demo.py:207-211.
         Sampling controls of the body prior as in s2g_body_pixel.generate: ``temperature`` (0 = greedy, no noise is
@@ -97,13 +98,18 @@ class WholeBody:
         ``temperature`` / ``top_k`` / ``top_p`` / ``min_p`` may each be given per clip (s2g_body_pixel.generate): one batch
         serves clips with different settings, on the overlapped and the sequential path alike.
         ``repetition_penalty`` / ``repetition_window`` / ``code_bias``: logit shaping of the body prior
-        (s2g_body_pixel.generate), on both paths."""
+        (s2g_body_pixel.generate), on both paths.
+        ``guidance`` with ``guide_mfcc`` ([B,64,M] or "silence"), ``guide_label`` and / or ``guide_style``: guided
+        sampling of the body prior (s2g_body_pixel.generate); with ``keep_logp`` the negative branches' log p is kept as
+        self.last_guide_logp."""
         B, _, M = mfcc.shape
         frame = wave.shape[1] * 30 // 16000
         T = self.e.latent_rows(M)
         shaping = shaping_kwargs(repetition_penalty, repetition_window, code_bias, B)
+        guide = guide_kwargs(guidance, guide_mfcc, guide_label, guide_style, keep_logp, self.e, B, M)
         ctl = sample_controls(temperature, top_k, keep_logp, top_p, min_p)
         ctl.update(shaping)
+        ctl.update(guide)
         want_kept = bool(ctl.get("want_kept"))
         if noise is not None and clip_seeds is not None:
             raise ValueError("WholeBody.generate: noise and clip_seeds are two noise sources; give one")
@@ -128,6 +134,7 @@ class WholeBody:
             self.last_codes = out[0]
             self.last_logp = out[2] if keep_logp else None
             self.last_kept = out[3] if want_kept else None
+            self.last_guide_logp = out[-1] if guide and keep_logp else None
             face = self.e.face_forward(wave, idz, frame)
             cur.wait_stream(self._side)
             body.record_stream(cur)                                      # allocated on the side stream, consumed here
@@ -137,7 +144,10 @@ class WholeBody:
                 self.last_kept.record_stream(cur)
             if keep_codes:
                 self.last_codes.record_stream(cur)
-            for t in (mfcc, label, noise, ctl.get("seeds"), ctl.get("anchors"), ctl.get("style"), ctl.get("code_bias")):
+            if self.last_guide_logp is not None:
+                self.last_guide_logp.record_stream(cur)
+            for t in (mfcc, label, noise, ctl.get("seeds"), ctl.get("anchors"), ctl.get("style"), ctl.get("code_bias"),
+                      ctl.get("guide_mfcc"), ctl.get("guide_label"), ctl.get("guide_style")):
                 if torch.is_tensor(t) and t.is_cuda:
                     t.record_stream(self._side)                          # allocated here, consumed on the side stream
             return self.e.assemble_pose(face, body, stand)
@@ -147,6 +157,7 @@ class WholeBody:
         self.last_codes = out[0]
         self.last_logp = out[2] if keep_logp else None
         self.last_kept = out[3] if want_kept else None
+        self.last_guide_logp = out[-1] if guide and keep_logp else None
         return self.e.assemble_pose(face, out[1], stand)
 
     def evaluate(self, bat):
@@ -184,7 +195,8 @@ class WholeBody:
 
     def generate_sharded(self, mfcc, wave, label, rank, world, noise_full=None, seed=None, stand=False, gather=True,
                          group=None, temperature=1.0, top_k=0, keep_logp=False, top_p=1.0, min_p=0.0, clip_seeds=None,
-                         anchors=None, style=None, repetition_penalty=1.0, repetition_window=8, code_bias=None):
+                         anchors=None, style=None, repetition_penalty=1.0, repetition_window=8, code_bias=None,
+                         guidance=None, guide_mfcc=None, guide_label=None, guide_style=None):
         """Multi-GPU form of ``generate`` whose RESULT DOES NOT DEPEND ON ``world`` (SURVEY.md §8e): the arguments are
         the FULL batch (host or device tensors, identical on every rank), the sampler noise is drawn for the full batch in
         the reference's order — ``noise_full`` [2T,B,2048], or drawn here from ``seed`` on this rank's device generator
@@ -200,7 +212,8 @@ class WholeBody:
         ``generate``): rank r passes its shard's rows.  Per-clip ``temperature`` / ``top_k`` / ``top_p`` / ``min_p`` (full
         batch, as in ``generate``): rank r passes its shard's values.  ``repetition_penalty`` / ``repetition_window`` (scalar
         or per clip) and ``code_bias`` ([2,2048] or [B,2,2048]) as in ``generate``: rank r passes its shard's values and bias
-        rows."""
+        rows.  ``guidance`` (scalar or per clip) and the negative conditioning (full batch, as in ``generate``): rank r
+        passes its shard's clips, each with its own negative branch, so a pair is never split across ranks."""
         B, _, M = mfcc.shape
         lo, hi = shard_range(B, rank, world)
         T = self.e.latent_rows(M)
@@ -224,6 +237,17 @@ class WholeBody:
             ctl.update(repetition_penalty=shape["repetition_penalty"], repetition_window=shape["repetition_window"])
             if code_bias is not None:
                 ctl["code_bias"] = check_code_bias(code_bias, B)[lo:hi]
+        if guidance is not None:
+            ctl["guidance"] = check_guidance(guidance, B)[lo:hi]
+            rows = lambda t: t if t is None or isinstance(t, str) else torch.as_tensor(t)[lo:hi]
+            ctl["guide_mfcc"] = rows(guide_mfcc)
+            if guide_label is not None:
+                gl = torch.as_tensor(guide_label).reshape(-1)
+                ctl["guide_label"] = gl.expand(B)[lo:hi] if gl.numel() == 1 else gl[lo:hi]
+            if guide_style is not None:
+                ctl["guide_style"] = check_style(guide_style, B, T, self.e.pixelcnn_ncls)[lo:hi]
+        else:
+            guide_kwargs(guidance, guide_mfcc, guide_label, guide_style)   # a negative conditioning alone raises
         if seeds is not None:
             ctl["clip_seeds"] = seeds[lo:hi]
         elif noise_full is None and sampled(temperature):
@@ -237,6 +261,8 @@ class WholeBody:
             local = torch.empty(0, frame, 265, device=self.device)
             self.last_logp = torch.empty(0, T, 2, device=self.device) if keep_logp else None
             self.last_kept = torch.empty(0, T, 2, dtype=torch.int32, device=self.device) if sc.get("want_kept") else None
+            self.last_guide_logp = (torch.empty(0, T, 2, device=self.device) if guidance is not None and keep_logp
+                                    else None)
         else:
             dev = lambda t: t[lo:hi].to(self.device, non_blocking=True)
             nz = None if noise_full is None else noise_full[:, lo:hi].to(self.device).contiguous()
