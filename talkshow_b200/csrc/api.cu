@@ -240,16 +240,10 @@ extern "C" int ts_vq_dim(ts_engine* e, int which) {
 }
 
 // ---- fused body path: audio encoder -> PixelCNN sampler -> two VQ decoders -------------------------
-// ctl = nullptr: the default sampler (ts_body_generate); else the sampling controls of ts_body_sample.
-// seeds (ts_body_sample_seeded): per-clip seeds in place of noise.  anchors (ts_body_sample_anchored): pinned draws.
-// style (ts_body_sample_styled): per-row speaker weights in place of label.  clip_ctl (ts_body_sample_clips): per-clip
-// controls (host, validated) in place of ctl's four.  clip_shape / code_bias (ts_body_sample_shaped): logit shaping.
-// guide (ts_body_sample_guided): B = 2P branches sampled in pairs; codes gets every branch, poses the P conditional ones.
+// d: the draw inputs (SampleCtl), the default sampler (ts_body_generate) when they are the defaults.  Guided (d.guide,
+// ts_body_sample_guided): B = 2P branches sampled in pairs; codes gets every branch, poses the P conditional ones.
 static void body_generate(ts_engine* e, const float* mfcc, const int64_t* label, const float* noise, int64_t* codes,
-                          float* poses, int B, int M, void* stream, const SampleCtl* ctl, const int64_t* seeds = nullptr,
-                          const int64_t* anchors = nullptr, const float* style = nullptr,
-                          const ts_clip_ctl* clip_ctl = nullptr, const ts_clip_shape* clip_shape = nullptr,
-                          const float* code_bias = nullptr, const float* guide = nullptr) {
+                          float* poses, int B, int M, void* stream, const SampleCtl& d = SampleCtl()) {
   ts::require_device(e);
   if (!e->conv || !e->conv->audio_loaded) fail(TS_ERR_NOT_LOADED, "audio encoder weights not loaded");
   if (!e->conv->vq[0].loaded || !e->conv->vq[1].loaded) fail(TS_ERR_NOT_LOADED, "vq weights not loaded");
@@ -266,11 +260,10 @@ static void body_generate(ts_engine* e, const float* mfcc, const int64_t* label,
     Act3 a = run_trunk(e, e->conv->audio, x, s);          // [B,T,256] channel-last, pad 1
     int64_t* idx = e->ws.alloc<int64_t>((size_t)B * T * 2);
     int64_t* idx_c = e->ws.alloc<int64_t>((size_t)B * T * 2);  // [2][B][T] column-split copy
-    pixelcnn_generate_act(e, a, label, noise, idx, nullptr, B, T, nullptr, 0, s, false, ctl, seeds, anchors, style, clip_ctl,
-                          clip_shape, code_bias, guide);
-    if (guide) split_guided_codes(e, idx, idx_c, B / 2, T, codes, s);   // decode the conditional branches only
+    pixelcnn_generate_act(e, a, label, noise, idx, nullptr, B, T, nullptr, 0, s, false, d);
+    if (d.guide) split_guided_codes(e, idx, idx_c, B / 2, T, codes, s);   // decode the conditional branches only
     else split_codes(e, idx, idx_c, B, T, codes, s);
-    const int Bd = guide ? B / 2 : B;
+    const int Bd = d.guide ? B / 2 : B;
     const int c0 = e->conv->vq[0].out_dim, c1 = e->conv->vq[1].out_dim;   // 39 + 90 (axis-angle) or 78 + 180 (6-D)
     // Small batches: each decoder is a chain of ~20 launches that fill a few SMs, so the hand decoder runs on a second
     // stream beside the body decoder (fork after the code split, join before the call returns to the caller's stream).
@@ -308,7 +301,7 @@ static void body_generate(ts_engine* e, const float* mfcc, const int64_t* label,
 extern "C" int ts_body_generate(ts_engine* e, const float* mfcc, const int64_t* label, const float* noise,
                                 int64_t* codes, float* poses, int B, int M, void* stream) {
   TS_API_BEGIN(e)
-  body_generate(e, mfcc, label, noise, codes, poses, B, M, stream, nullptr);
+  body_generate(e, mfcc, label, noise, codes, poses, B, M, stream);
   TS_API_END(e)
 }
 
@@ -323,7 +316,7 @@ extern "C" int ts_body_sample_ctl(ts_engine* e, const float* mfcc, const int64_t
   TS_API_BEGIN(e)
   const SampleCtl c = sample_ctl_of(ctl);
   check_sample_ctl(c, noise);
-  body_generate(e, mfcc, label, noise, codes, poses, B, M, stream, &c);
+  body_generate(e, mfcc, label, noise, codes, poses, B, M, stream, c);
   TS_API_END(e)
 }
 
@@ -331,14 +324,15 @@ extern "C" int ts_body_sample_seeded(ts_engine* e, const float* mfcc, const int6
                                      float* poses, int B, int M, const ts_sample_ctl* ctl, void* stream) {
   TS_API_BEGIN(e)
   ts::require_device(e);
+  SampleCtl c;
   if (ctl) {
-    const SampleCtl c = sample_ctl_of(ctl);
+    c = sample_ctl_of(ctl);
     check_sample_ctl(c, nullptr, seeds);
-    body_generate(e, mfcc, label, nullptr, codes, poses, B, M, stream, &c, seeds);
-  } else {
-    if (!seeds) fail(TS_ERR_INVALID, "ts_body_sample_seeded: seeds is NULL (only greedy decoding runs without)");
-    body_generate(e, mfcc, label, nullptr, codes, poses, B, M, stream, nullptr, seeds);
+  } else if (!seeds) {
+    fail(TS_ERR_INVALID, "ts_body_sample_seeded: seeds is NULL (only greedy decoding runs without)");
   }
+  c.seeds = seeds;
+  body_generate(e, mfcc, label, nullptr, codes, poses, B, M, stream, c);
   TS_API_END(e)
 }
 
@@ -353,7 +347,8 @@ extern "C" int ts_body_sample_anchored(ts_engine* e, const float* mfcc, const in
     check_sample_ctl(c, noise, seeds);
   }
   check_anchored_source(ctl ? &c : nullptr, noise, seeds, "ts_body_sample_anchored");
-  body_generate(e, mfcc, label, noise, codes, poses, B, M, stream, ctl ? &c : nullptr, seeds, anchors);
+  c.seeds = seeds; c.anchors = anchors;
+  body_generate(e, mfcc, label, noise, codes, poses, B, M, stream, c);
   TS_API_END(e)
 }
 
@@ -370,7 +365,8 @@ extern "C" int ts_body_sample_styled(ts_engine* e, const float* mfcc, const int6
     check_sample_ctl(c, noise, seeds);
   }
   check_anchored_source(ctl ? &c : nullptr, noise, seeds, "ts_body_sample_styled");
-  body_generate(e, mfcc, label, noise, codes, poses, B, M, stream, ctl ? &c : nullptr, seeds, anchors, style);
+  c.seeds = seeds; c.anchors = anchors; c.style = style;
+  body_generate(e, mfcc, label, noise, codes, poses, B, M, stream, c);
   TS_API_END(e)
 }
 
@@ -388,7 +384,8 @@ extern "C" int ts_body_sample_clips(ts_engine* e, const float* mfcc, const int64
   check_clip_ctl(clip_ctl, B, noise, seeds, "ts_body_sample_clips");
   SampleCtl c;   // logp_out / kept_out of ctl; the draws' controls come from clip_ctl
   if (ctl) { c.logp_out = ctl->logp_out; c.kept_out = ctl->kept_out; }
-  body_generate(e, mfcc, label, noise, codes, poses, B, M, stream, &c, seeds, anchors, style, clip_ctl);
+  c.seeds = seeds; c.anchors = anchors; c.style = style; c.clip_ctl = clip_ctl;
+  body_generate(e, mfcc, label, noise, codes, poses, B, M, stream, c);
   TS_API_END(e)
 }
 
@@ -404,8 +401,9 @@ extern "C" int ts_body_sample_shaped(ts_engine* e, const float* mfcc, const int6
   if (B <= 0) fail(TS_ERR_INVALID, "ts_body_sample_shaped: B=%d", B);
   check_style(e, label, style, ncls, "ts_body_sample_shaped");
   if (clip_shape) check_clip_shape(clip_shape, B, "ts_body_sample_shaped");
-  const SampleCtl c = shaped_ctl(ctl, clip_ctl, B, noise, seeds, "ts_body_sample_shaped");
-  body_generate(e, mfcc, label, noise, codes, poses, B, M, stream, &c, seeds, anchors, style, clip_ctl, clip_shape, code_bias);
+  SampleCtl c = shaped_ctl(ctl, clip_ctl, B, noise, seeds, "ts_body_sample_shaped");
+  c.seeds = seeds; c.anchors = anchors; c.style = style; c.clip_ctl = clip_ctl; c.clip_shape = clip_shape; c.code_bias = code_bias;
+  body_generate(e, mfcc, label, noise, codes, poses, B, M, stream, c);
   TS_API_END(e)
 }
 
@@ -421,8 +419,9 @@ extern "C" int ts_body_sample_guided(ts_engine* e, const float* mfcc, const int6
   check_style(e, label, style, ncls, "ts_body_sample_guided");
   check_guidance(guidance, P, "ts_body_sample_guided");
   if (clip_shape) check_clip_shape(clip_shape, P, "ts_body_sample_guided");
-  const SampleCtl c = shaped_ctl(ctl, clip_ctl, P, noise, seeds, "ts_body_sample_guided");
-  body_generate(e, mfcc, label, noise, codes, poses, 2 * P, M, stream, &c, seeds, anchors, style, clip_ctl, clip_shape,
-                code_bias, guidance);
+  SampleCtl c = shaped_ctl(ctl, clip_ctl, P, noise, seeds, "ts_body_sample_guided");
+  c.seeds = seeds; c.anchors = anchors; c.style = style; c.clip_ctl = clip_ctl; c.clip_shape = clip_shape; c.code_bias = code_bias;
+  c.guide = guidance;
+  body_generate(e, mfcc, label, noise, codes, poses, 2 * P, M, stream, c);
   TS_API_END(e)
 }

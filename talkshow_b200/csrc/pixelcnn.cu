@@ -466,42 +466,23 @@ struct PixArgs {
   int B, T0, Ttot, log_r0, L, nstages, ncta, fused;
   unsigned long long* trace;   // [nstages][ncta][4] globaltimer stamps of row trace_row (debug builds of the kernel only)
   int trace_row;
-  // sampling controls, read by the WARP instantiations only (kept last: the fields above keep their offsets)
-  float temperature;
-  int top_k;
-  float* logp_out;     // [B][Ttot-T0][2] or null
-  float top_p, min_p;
-  int* kept_out;       // [B][Ttot-T0][2] or null
-  // seeded sampling (ts_pixelcnn_sample_seeded): [B] per-clip seeds; the draw's q comes from seeded_q, noise is unread
-  const int64_t* seeds;
-  // anchored sampling (ts_pixelcnn_sample_anchored), read by the WARP instantiations only: [B][Ttot-T0][2], a value in
-  // [0, 2048) pins the draw to that code, anything else samples it; or null
-  const int64_t* anchors;
-  // styled sampling (ts_pixelcnn_sample_styled), read by the WARP instantiations only: [B][Ttot][ncls] speaker weights per
-  // row, blended from cls_w [L][ncls][2D] at every gate in place of the CLS arena (style_pair); or null
-  const float* style;
+  // the draw inputs (device copies).  The default kernels read seeds only; every other field is read by the WARP
+  // instantiations.  Indexed by the global clip index, or in a guided call by the pair (draw_index).
+  SampleCtl draw;
+  // styled sampling, read by the WARP instantiations only: the class embeddings [L][ncls][2D] that draw.style blends at
+  // every gate in place of the CLS arena (style_pair).  After `draw`, so that draw.seeds keeps its offset.
   const float* cls_w;
   int ncls;
-  // per-clip controls (ts_pixelcnn_sample_clips), read by the WARP instantiations only: [B] (device), indexed by the
-  // global clip index; or null (the scalar controls above)
-  const ts_clip_ctl* clip_ctl;
-  // logit shaping (ts_pixelcnn_sample_shaped), read by the WARP instantiations only, by global clip index: [B] (device)
-  // repetition penalty and window, or null (theta 1); [B][2][2048] (device) code bias, or null
-  const ts_clip_shape* clip_shape;
-  const float* code_bias;
-  // guided sampling (ts_pixelcnn_sample_guided), read by the WARP instantiations only: [B / 2] (device) guidance scale of
-  // each pair of samples (2p conditional, 2p + 1 negative); every draw input above is then indexed by the pair; or null
-  const float* guide;
 };
 
 // The draw-input index of sample m (WARP instantiations only): in a guided call samples 2p and 2p + 1 are the two branches
 // of pair p and read pair p's noise or seed, controls, anchors, shaping and scale; otherwise sample m's own.
 template <class Args>
 __device__ __forceinline__ int draw_index(const Args& A, int m) {
-  return A.guide ? m >> 1 : m;
+  return A.draw.guide ? m >> 1 : m;
 }
 
-// The sampling controls of clip m (global index): its entry of A.clip_ctl, else the call's scalar controls.  Every draw
+// The sampling controls of clip m (global index): its entry of A.draw.clip_ctl, else the call's scalar controls.  Every draw
 // of one clip runs in one CTA, so the value is uniform over the threads that call draw_controlled together.
 static_assert(sizeof(ts_clip_ctl) == 16, "ts_clip_ctl is read as one 16-byte load");
 struct DrawCtl {
@@ -511,16 +492,16 @@ struct DrawCtl {
 };
 template <class Args>
 __device__ __forceinline__ DrawCtl draw_ctl(const Args& A, int m) {
-  if (A.clip_ctl) {
-    const int4 v = __ldg(reinterpret_cast<const int4*>(A.clip_ctl) + m);
+  if (A.draw.clip_ctl) {
+    const int4 v = __ldg(reinterpret_cast<const int4*>(A.draw.clip_ctl) + m);
     return {__int_as_float(v.x), v.y, __int_as_float(v.z), __int_as_float(v.w)};
   }
-  return {A.temperature, A.top_k, A.top_p, A.min_p};
+  return {A.draw.temperature, A.draw.top_k, A.draw.top_p, A.draw.min_p};
 }
 // The temperature of clip m alone (the noise prefetch before the barrier wait: a greedy clip reads no noise).
 template <class Args>
 __device__ __forceinline__ float draw_temperature(const Args& A, int m) {
-  return A.clip_ctl ? __ldg(&A.clip_ctl[m].temperature) : A.temperature;
+  return A.draw.clip_ctl ? __ldg(&A.draw.clip_ctl[m].temperature) : A.draw.temperature;
 }
 
 // ---- logit shaping: the rule of ts_pixelcnn_sample_shaped (include/talkshow_b200.h) --------------------------------
@@ -535,8 +516,8 @@ struct ShapeCtl {
 };
 template <class Args>
 __device__ __forceinline__ ShapeCtl shape_ctl(const Args& A, int m) {
-  if (!A.clip_shape) return {1.f, 0};
-  const int2 v = __ldg(reinterpret_cast<const int2*>(A.clip_shape) + m);
+  if (!A.draw.clip_shape) return {1.f, 0};
+  const int2 v = __ldg(reinterpret_cast<const int2*>(A.draw.clip_shape) + m);
   return {__int_as_float(v.x), v.y};
 }
 
@@ -563,8 +544,8 @@ __device__ __forceinline__ void shape_stage(const Args& A, int m, int r, int c, 
       if (code >= 0 && code < PIX_NCODE) atomicOr(&bits[code >> 5], 1u << (code & 31));
     }
   }
-  if (A.code_bias) {
-    const float* b = A.code_bias + ((size_t)draw_index(A, m) * 2 + c) * PIX_NCODE;
+  if (A.draw.code_bias) {
+    const float* b = A.draw.code_bias + ((size_t)draw_index(A, m) * 2 + c) * PIX_NCODE;
 #pragma unroll
     for (int j = 0; j < 8; ++j) red[SHAPE_BIAS + tid + 256 * j] = __ldg(b + tid + 256 * j);
   }
@@ -584,17 +565,17 @@ __device__ __forceinline__ bool shape_logits(const Args& A, int m, const float* 
       if ((bits[(tid >> 5) + 8 * j] >> (tid & 31)) & 1u)
         l[j] = l[j] > 0.f ? __fdiv_rn(l[j], sc.theta) : __fmul_rn(l[j], sc.theta);
   }
-  if (A.code_bias) {
+  if (A.draw.code_bias) {
 #pragma unroll
     for (int j = 0; j < 8; ++j) l[j] = __fadd_rn(l[j], red[SHAPE_BIAS + tid + 256 * j]);
   }
-  return sc.theta != 1.f || A.code_bias != nullptr;
+  return sc.theta != 1.f || A.draw.code_bias != nullptr;
 }
 
-// The speaker weights of row r of clip m (global index) under A.style, or null for a padding sample (m >= B).
+// The speaker weights of row r of clip m (global index) under A.draw.style, or null for a padding sample (m >= B).
 template <class Args>
 __device__ __forceinline__ const float* style_row(const Args& A, int m, int r) {
-  return m < A.B ? A.style + ((size_t)m * A.Ttot + r) * A.ncls : nullptr;
+  return m < A.B ? A.draw.style + ((size_t)m * A.Ttot + r) * A.ncls : nullptr;
 }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -709,96 +690,6 @@ __device__ __forceinline__ int resolve_segments(const PixTask& t, int pass, int 
   return 0;
 }
 
-// partial products of this CTA's rows over the warp's K slice; lane owns samples 2*lane, 2*lane+1
-template <int RC>
-__device__ __forceinline__ void mm_rows(const float* __restrict__ Wsm, int K, const int* seg, const float* arena,
-                                        float* red, int warp, int lane) {
-  constexpr int MB = 64;   // lane owns samples 2*lane, 2*lane+1
-  float2 acc[4 * RC];
-#pragma unroll
-  for (int j = 0; j < 4 * RC; ++j) acc[j] = make_float2(0.f, 0.f);
-  const int kper = K >> 3;  // K is a multiple of 256 -> 32 | kper
-  // K slices are rotated by CTA so that the CTAs do not all pull the same L2 lines at the same time;
-  // partials are stored by slice index, so the reduction order does not depend on the rotation
-  const int slice = (warp + blockIdx.x) & 7;
-  const int kbeg = slice * kper;
-  constexpr int U = 32;   // K = 256 stages issue their whole K slice in one batch of loads
-  for (int k0 = kbeg; k0 < kbeg + kper; k0 += U) {
-    const float* base = arena + seg[k0 >> 8] + ((k0 & 255) * MB) + lane * 2;
-    float2 x[U];
-#pragma unroll
-    for (int u = 0; u < U; ++u) x[u] = __ldcg(reinterpret_cast<const float2*>(base + u * MB));
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const float4* w4 = reinterpret_cast<const float4*>(Wsm + (size_t)(k0 + u) * (4 * RC));
-#pragma unroll
-      for (int rc = 0; rc < RC; ++rc) {
-        float4 w = w4[rc];
-        acc[rc * 4 + 0].x = fmaf(w.x, x[u].x, acc[rc * 4 + 0].x); acc[rc * 4 + 0].y = fmaf(w.x, x[u].y, acc[rc * 4 + 0].y);
-        acc[rc * 4 + 1].x = fmaf(w.y, x[u].x, acc[rc * 4 + 1].x); acc[rc * 4 + 1].y = fmaf(w.y, x[u].y, acc[rc * 4 + 1].y);
-        acc[rc * 4 + 2].x = fmaf(w.z, x[u].x, acc[rc * 4 + 2].x); acc[rc * 4 + 2].y = fmaf(w.z, x[u].y, acc[rc * 4 + 2].y);
-        acc[rc * 4 + 3].x = fmaf(w.w, x[u].x, acc[rc * 4 + 3].x); acc[rc * 4 + 3].y = fmaf(w.w, x[u].y, acc[rc * 4 + 3].y);
-      }
-    }
-  }
-#pragma unroll
-  for (int j = 0; j < 4 * RC; ++j)
-    *reinterpret_cast<float2*>(&red[(slice * PIX_MAXROWS + j) * MB + lane * 2]) = acc[j];
-}
-
-// Same partial products (same per-accumulator summation order -> bit-identical), software-pipelined: the
-// activation loads form a ring of 4 groups x 8 rows; a group is re-issued for k+32 as soon as its FMAs are
-// done, so every warp keeps 24-32 L2 loads in flight while it computes instead of alternating a load burst
-// and an FMA burst (which also synchronises the L2 traffic of all CTAs into bursts).
-template <int RC, int G>
-__device__ __forceinline__ void mm_rows_pipe(const float* __restrict__ Wsm, int K, const int* seg, const float* arena,
-                                             float* red, int warp, int lane) {
-  constexpr int MB = 64;
-  float2 acc[4 * RC];
-#pragma unroll
-  for (int j = 0; j < 4 * RC; ++j) acc[j] = make_float2(0.f, 0.f);
-  const int kper = K >> 3;  // multiple of 32
-  const int slice = (warp + blockIdx.x) & 7;
-  const int kbeg = slice * kper, kend = kbeg + kper;
-  constexpr int GS = 8;
-  float2 x[G][GS];
-#pragma unroll
-  for (int g = 0; g < G; ++g) {   // kper is a multiple of G * GS = 32
-    const int k = kbeg + g * GS;
-    const float* base = arena + seg[k >> 8] + ((k & 255) * MB) + lane * 2;
-#pragma unroll
-    for (int u = 0; u < GS; ++u) x[g][u] = __ldcg(reinterpret_cast<const float2*>(base + u * MB));
-  }
-  for (int k0 = kbeg; k0 < kend; k0 += G * GS) {
-    const bool more = k0 + G * GS < kend;
-#pragma unroll
-    for (int g = 0; g < G; ++g) {
-#pragma unroll
-      for (int u = 0; u < GS; ++u) {
-        const float4* w4 = reinterpret_cast<const float4*>(Wsm + (size_t)(k0 + g * GS + u) * (4 * RC));
-        const float2 xv = x[g][u];
-#pragma unroll
-        for (int rc = 0; rc < RC; ++rc) {
-          float4 w = w4[rc];
-          acc[rc * 4 + 0].x = fmaf(w.x, xv.x, acc[rc * 4 + 0].x); acc[rc * 4 + 0].y = fmaf(w.x, xv.y, acc[rc * 4 + 0].y);
-          acc[rc * 4 + 1].x = fmaf(w.y, xv.x, acc[rc * 4 + 1].x); acc[rc * 4 + 1].y = fmaf(w.y, xv.y, acc[rc * 4 + 1].y);
-          acc[rc * 4 + 2].x = fmaf(w.z, xv.x, acc[rc * 4 + 2].x); acc[rc * 4 + 2].y = fmaf(w.z, xv.y, acc[rc * 4 + 2].y);
-          acc[rc * 4 + 3].x = fmaf(w.w, xv.x, acc[rc * 4 + 3].x); acc[rc * 4 + 3].y = fmaf(w.w, xv.y, acc[rc * 4 + 3].y);
-        }
-      }
-      if (more) {
-        const int k = k0 + G * GS + g * GS;
-        const float* base = arena + seg[k >> 8] + ((k & 255) * MB) + lane * 2;
-#pragma unroll
-        for (int u = 0; u < GS; ++u) x[g][u] = __ldcg(reinterpret_cast<const float2*>(base + u * MB));
-      }
-    }
-  }
-#pragma unroll
-  for (int j = 0; j < 4 * RC; ++j)
-    *reinterpret_cast<float2*>(&red[(slice * PIX_MAXROWS + j) * MB + lane * 2]) = acc[j];
-}
-
 // Two IEEE fp32 FMAs on a register pair: the accumulator pair is the lane's two samples, the weight is the broadcast
 // operand.  The pair layout keeps 64-bit loads of the activations; the pack / unpack moves compile to nothing.
 __device__ __forceinline__ void fma2(unsigned long long& acc, float w, unsigned long long x) {
@@ -810,6 +701,11 @@ __device__ __forceinline__ void fma2(unsigned long long& acc, float w, unsigned 
   asm("mov.b64 %0, {%1, %2};" : "=l"(acc) : "f"(a0), "f"(a1));
 }
 
+// Partial products of this CTA's rows over the warp's K slice (64-sample tile): lane owns samples 2*lane, 2*lane+1, every
+// accumulator sums its K slice in k order with one fmaf per term.  The activation loads form a ring of G groups x 8 rows;
+// a group is re-issued for k+32 as soon as its FMAs are done, so every warp keeps 24-32 L2 loads in flight while it
+// computes instead of alternating a load burst and an FMA burst (which also synchronises the L2 traffic of all CTAs into
+// bursts).
 template <int RC, int G>
 __device__ __forceinline__ void mm_rows_pipe2(const float* __restrict__ Wsm, int K, const int* seg, const float* arena,
                                               float* red, int warp, int lane) {
@@ -818,6 +714,8 @@ __device__ __forceinline__ void mm_rows_pipe2(const float* __restrict__ Wsm, int
 #pragma unroll
   for (int j = 0; j < 4 * RC; ++j) acc[j] = 0ull;
   const int kper = K >> 3;  // multiple of 32
+  // K slices are rotated by CTA so that the CTAs do not all pull the same L2 lines at the same time;
+  // partials are stored by slice index, so the reduction order does not depend on the rotation
   const int slice = (warp + blockIdx.x) & 7;
   const int kbeg = slice * kper, kend = kbeg + kper;
   constexpr int GS = 8;
@@ -993,10 +891,10 @@ __device__ __forceinline__ EpiPre prefetch_epilogue(const PixTask& t, const PixA
   return p;
 }
 
-// WARP: a styled call (A.style) blends each gate's class term from row r's speaker weights; every gate a stage computes
+// WARP: a styled call (A.draw.style) blends each gate's class term from row r's speaker weights; every gate a stage computes
 // at latent row r belongs to a position of row r (the vertical stack of row r reads rows < r only, the horizontal pass and
 // the forced prefix rows run at their own row), so row r of the schedule is the row of every gate here.
-template <int PIPE, int MB, bool S2 = false, bool WARP = false>
+template <int MB, bool S2 = false, bool WARP = false>
 __device__ void run_matmul_task(const PixTask& t, const PixArgs& A, int r, const float* Wsm, float* red, const EpiPre& pre) {
   constexpr int SEG = PIX_D * MB;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -1027,26 +925,12 @@ __device__ void run_matmul_task(const PixTask& t, const PixArgs& A, int r, const
             default: mm_rows_small<4, MB, 4>(Wsm, t.K, s_seg, arena, red, warp, lane); break;
           }
         }
-      } else if constexpr (PIPE == 5) {
+      } else {
         switch (t.rpad >> 2) {
           case 1: mm_rows_pipe2<1, 4>(Wsm, t.K, s_seg, arena, red, warp, lane); break;
           case 2: mm_rows_pipe2<2, 4>(Wsm, t.K, s_seg, arena, red, warp, lane); break;
           case 3: mm_rows_pipe2<3, 4>(Wsm, t.K, s_seg, arena, red, warp, lane); break;
           default: mm_rows_pipe2<4, 4>(Wsm, t.K, s_seg, arena, red, warp, lane); break;
-        }
-      } else if constexpr (PIPE > 0) {
-        switch (t.rpad >> 2) {
-          case 1: mm_rows_pipe<1, PIPE>(Wsm, t.K, s_seg, arena, red, warp, lane); break;
-          case 2: mm_rows_pipe<2, PIPE>(Wsm, t.K, s_seg, arena, red, warp, lane); break;
-          case 3: mm_rows_pipe<3, PIPE>(Wsm, t.K, s_seg, arena, red, warp, lane); break;
-          default: mm_rows_pipe<4, PIPE>(Wsm, t.K, s_seg, arena, red, warp, lane); break;
-        }
-      } else {
-        switch (t.rpad >> 2) {
-          case 1: mm_rows<1>(Wsm, t.K, s_seg, arena, red, warp, lane); break;
-          case 2: mm_rows<2>(Wsm, t.K, s_seg, arena, red, warp, lane); break;
-          case 3: mm_rows<3>(Wsm, t.K, s_seg, arena, red, warp, lane); break;
-          default: mm_rows<4>(Wsm, t.K, s_seg, arena, red, warp, lane); break;
         }
       }
     }
@@ -1062,7 +946,7 @@ __device__ void run_matmul_task(const PixTask& t, const PixArgs& A, int r, const
         const float* cls = arena + a.CLS + (t.layer * 2) * SEG;
         float ct = cls[ax<MB>(q, m)], cs = cls[ax<MB>(PIX_D + q, m)];
         if constexpr (WARP) {
-          if (A.style) style_pair(A.cls_w + (size_t)t.layer * A.ncls * 2 * PIX_D, style_row(A, m, r), A.ncls, PIX_D, q, ct, cs);
+          if (A.draw.style) style_pair(A.cls_w + (size_t)t.layer * A.ncls * 2 * PIX_D, style_row(A, m, r), A.ncls, PIX_D, q, ct, cs);
         }
         if (t.epi == EPI_HGATE || t.epi == EPI_HGATE2) {
           const float* v2h = arena + a.V2H + ((t.layer * 2 + t.col) * 2) * SEG;
@@ -1428,8 +1312,8 @@ __device__ __forceinline__ void draw_pinned(const float (&l)[8], long long code,
 // Any other value samples, so malformed device data never reaches the embedding gather.
 template <class Args>
 __device__ __forceinline__ long long anchor_of(const Args& A, size_t at) {
-  if (!A.anchors) return -1;
-  const long long a = __ldg(A.anchors + at);
+  if (!A.draw.anchors) return -1;
+  const long long a = __ldg(A.draw.anchors + at);
   return (a >= 0 && a < PIX_NCODE) ? a : -1;
 }
 
@@ -1466,36 +1350,25 @@ __device__ __forceinline__ void seeded_q(int64_t seed, int r, int c, int tid, fl
   }
 }
 
-// The noise of draw (r, c) of sample m (global clip index): computed from A.seeds, else read from A.noise.
-template <class Args>
+// The noise of draw (r, c) of sample m (global clip index): computed from A.draw.seeds, else read from A.noise.  The WARP
+// kernels read by draw_index: a guided call's pair p = m >> 1 reads seeds[p], or column p of noise [2T][B / 2][2048].
+// The guided read is its own branch: a select on the index changes the code of the WARP kernels.
+template <bool WARP, class Args>
 __device__ __forceinline__ void draw_noise(const Args& A, int r, int c, int m, float (&q)[8]) {
   const int tid = threadIdx.x;
-  if (A.seeds) {
-    seeded_q(A.seeds[m], r, c, tid, q);
-  } else {
-    const float* src = A.noise + ((size_t)(2 * (r - A.T0) + c) * A.B + m) * PIX_NCODE;
+  auto read = [&](int d, bool pair) {
+    if (A.draw.seeds) {
+      seeded_q(A.draw.seeds[d], r, c, tid, q);
+    } else {
+      const float* src = A.noise + ((size_t)(2 * (r - A.T0) + c) * (pair ? A.B >> 1 : A.B) + d) * PIX_NCODE;
 #pragma unroll
-    for (int j = 0; j < 8; ++j) q[j] = __ldcs(src + tid + 256 * j);
-  }
-}
-// draw_noise of the WARP kernels: a guided call's pair p = m >> 1 (draw_index) reads seeds[p], or column p of noise
-// [2T][B / 2][2048]; every other call is draw_noise.
-template <bool WARP, class Args>
-__device__ __forceinline__ void draw_noise_of(const Args& A, int r, int c, int m, float (&q)[8]) {
-  if constexpr (WARP) {
-    if (A.guide) {
-      const int tid = threadIdx.x, p = m >> 1;
-      if (A.seeds) {
-        seeded_q(A.seeds[p], r, c, tid, q);
-      } else {
-        const float* src = A.noise + ((size_t)(2 * (r - A.T0) + c) * (A.B >> 1) + p) * PIX_NCODE;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) q[j] = __ldcs(src + tid + 256 * j);
-      }
-      return;
+      for (int j = 0; j < 8; ++j) q[j] = __ldcs(src + tid + 256 * j);
     }
+  };
+  if constexpr (WARP) {
+    if (A.draw.guide) { read(draw_index(A, m), true); return; }
   }
-  draw_noise(A, r, c, m, q);
+  read(m, false);
 }
 
 // The guided logits of branch m's draw (ts_pixelcnn_sample_guided), in place of its raw logits l: with l_c the raw logits
@@ -1506,7 +1379,7 @@ __device__ __forceinline__ void draw_noise_of(const Args& A, int r, int c, int m
 template <class Args>
 __device__ __forceinline__ void guide_logits(const Args& A, int m, const float* partner, int stride, float (&l)[8]) {
   const int tid = threadIdx.x;
-  const float s = __fsub_rn(__ldg(A.guide + (m >> 1)), 1.f);
+  const float s = __fsub_rn(__ldg(A.draw.guide + (m >> 1)), 1.f);
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     const float o = __ldcg(partner + (size_t)(tid + 256 * j) * stride);
@@ -1515,16 +1388,19 @@ __device__ __forceinline__ void guide_logits(const Args& A, int m, const float* 
   }
 }
 
-// softmax over 2048 logits + categorical draw = argmax(p / q) (ATen multinomial, num_samples = 1),
-// then embedding gather of the sampled code into the E ring.  One CTA per sample.
-// QPRE (persistent kernel): the sampler noise of this position was loaded (or, seeded, computed) before the grid-barrier
-// wait (it is an input of the call, independent of every stage) and arrives in qpre[8].  Otherwise draw_noise here.
-// WARP: the draw applies the sampling controls of A (draw_controlled); otherwise the default draw below.
-template <int MB, bool QPRE = false, bool WARP = false>
-__device__ void run_sample_task(const PixTask& t, const PixArgs& A, int r, int m, float* red, const float* qpre = nullptr) {
-  constexpr int SEG = PIX_D * MB;
+// The draw of one sample stage, shared by both executors: softmax over the 2048 logits + categorical draw = argmax(p / q)
+// (ATen multinomial, num_samples = 1) with first-index ties.  One CTA per sample; its 256 threads, synchronised by `bar`,
+// own codes tid + 256 j.  logit(j): the address of code tid + 256 j in the sample's LOG slot (each executor keeps its own
+// address arithmetic, which the register allocation of its kernels depends on); partner: code 0 of branch m ^ 1's slot,
+// `stride` floats between codes (read by a guided draw only); m: the global clip index; q: the draw's noise, loaded (or,
+// seeded, computed) before the stage barrier (unread by forced rows and by pinned and greedy draws).  Rows r < T0 take
+// pre's code.  Writes logits_out and idx_out, and (WARP) logp_out and kept_out; returns the code.
+// WARP: the draw applies the anchors, controls, shaping and guidance of A.draw (draw_controlled); otherwise the default
+// draw below.
+template <bool WARP, class Args, class Bar, class Logit>
+__device__ __forceinline__ long long sample_draw(const Args& A, Bar bar, Logit logit, const float* partner, int stride, int m,
+                                                 int r, int c, float* red, const float (&q)[8]) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int c = t.col;
   float* sf = red;                                  // [8] scratch
   int* si = reinterpret_cast<int*>(red + 16);       // [8] scratch
   long long* scode = reinterpret_cast<long long*>(red + 32);
@@ -1533,7 +1409,7 @@ __device__ void run_sample_task(const PixTask& t, const PixArgs& A, int r, int m
   float l[8];
   if (have_logits) {
 #pragma unroll
-    for (int j = 0; j < 8; ++j) l[j] = __ldcg(A.arena + A.lay.LOG + ax<MB>(tid + 256 * j, m));
+    for (int j = 0; j < 8; ++j) l[j] = __ldcg(logit(j));
     if (A.logits_out) {
       float* dst = A.logits_out + ((size_t)(2 * (r - A.log_r0) + c) * A.B + m) * PIX_NCODE;
 #pragma unroll
@@ -1544,31 +1420,24 @@ __device__ void run_sample_task(const PixTask& t, const PixArgs& A, int r, int m
   if constexpr (WARP) {
     if (!forced) {
       const size_t at = ((size_t)m * (A.Ttot - A.T0) + (r - A.T0)) * 2 + c;
-      const int d = draw_index(A, m);   // m, or a guided call's pair
+      // m, or a guided call's pair (its branches 2d, 2d + 1 share the tile or cluster: the cluster's MB is even)
+      const int d = draw_index(A, m);
       const long long pin = anchor_of(A, ((size_t)d * (A.Ttot - A.T0) + (r - A.T0)) * 2 + c);   // uniform branch
       if (pin >= 0) {
         code = pin;
-        draw_pinned(l, code, red, A.logp_out ? A.logp_out + at : nullptr, A.kept_out ? A.kept_out + at : nullptr, CtaBar());
+        draw_pinned(l, code, red, A.draw.logp_out ? A.draw.logp_out + at : nullptr,
+                    A.draw.kept_out ? A.draw.kept_out + at : nullptr, bar);
       } else {
         const DrawCtl dc = draw_ctl(A, d);   // clip m's (pair d's) controls: the whole CTA serves clip m
-        float qv[8];
-        if (dc.temperature > 0.f) {
-          if (QPRE) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) qv[j] = qpre[j];
-          } else {
-            draw_noise_of<true>(A, r, c, m, qv);
-          }
-        }
-        if (A.guide) guide_logits(A, m, A.arena + A.lay.LOG + (m ^ 1), MB, l);
-        const bool shaped = shape_logits(A, m, red, l) || A.guide;
-        float* logp = A.logp_out ? A.logp_out + at : nullptr;
-        code = draw_controlled(l, qv, dc.temperature, dc.top_k, dc.top_p, dc.min_p, red, shaped ? nullptr : logp,
-                               A.kept_out ? A.kept_out + at : nullptr, CtaBar());
+        if (A.draw.guide) guide_logits(A, m, partner, stride, l);
+        const bool shaped = shape_logits(A, m, red, l) || A.draw.guide;   // staged before the stage barrier
+        float* logp = A.draw.logp_out ? A.draw.logp_out + at : nullptr;
+        code = draw_controlled(l, q, dc.temperature, dc.top_k, dc.top_p, dc.min_p, red, shaped ? nullptr : logp,
+                               A.draw.kept_out ? A.draw.kept_out + at : nullptr, bar);
         if (shaped && logp) {   // log p under the branch's raw prior: the LOG slot still holds its unshaped logits
 #pragma unroll
-          for (int j = 0; j < 8; ++j) l[j] = __ldcg(A.arena + A.lay.LOG + ax<MB>(tid + 256 * j, m));
-          draw_pinned(l, code, red, logp, nullptr, CtaBar());
+          for (int j = 0; j < 8; ++j) l[j] = __ldcg(logit(j));
+          draw_pinned(l, code, red, logp, nullptr, bar);
         }
       }
     } else {
@@ -1580,54 +1449,59 @@ __device__ void run_sample_task(const PixTask& t, const PixArgs& A, int r, int m
     for (int j = 1; j < 8; ++j) mx = fmaxf(mx, l[j]);
     for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
     if (lane == 0) sf[warp] = mx;
-    __syncthreads();
+    bar();
     mx = sf[0];
 #pragma unroll
     for (int w = 1; w < 8; ++w) mx = fmaxf(mx, sf[w]);
-    __syncthreads();
+    bar();
     float ex[8], sum = 0.f;
 #pragma unroll
     for (int j = 0; j < 8; ++j) { ex[j] = expf(l[j] - mx); sum += ex[j]; }
     for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
     if (lane == 0) sf[warp] = sum;
-    __syncthreads();
+    bar();
     sum = sf[0];
 #pragma unroll
     for (int w = 1; w < 8; ++w) sum += sf[w];
-    __syncthreads();
-    float qv[8];
-    if (QPRE) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) qv[j] = qpre[j];
-    } else {
-      draw_noise(A, r, c, m, qv);
-    }
+    bar();
     float bv = -INFINITY;
     int bi = 0x7fffffff;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      int n = tid + 256 * j;
-      float v = (ex[j] / sum) / qv[j];
+      const int n = tid + 256 * j;
+      const float v = (ex[j] / sum) / q[j];
       if (v > bv || (v == bv && n < bi)) { bv = v; bi = n; }
     }
     for (int o = 16; o > 0; o >>= 1) {
-      float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-      int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+      const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
       if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
     }
     if (lane == 0) { sf[warp] = bv; si[warp] = bi; }
-    __syncthreads();
+    bar();
     if (tid == 0) {
       for (int w = 1; w < 8; ++w)
         if (sf[w] > bv || (sf[w] == bv && si[w] < bi)) { bv = sf[w]; bi = si[w]; }
       *scode = bi;
     }
-    __syncthreads();
+    bar();
     code = *scode;
   } else {
     code = A.pre[((size_t)m * A.T0 + r) * 2 + c];
   }
   if (r >= A.T0 && tid == 0) A.idx_out[((size_t)m * (A.Ttot - A.T0) + (r - A.T0)) * 2 + c] = code;
+  return code;
+}
+
+// The sample stage of the grid-wide executor: sample_draw, then the embedding gather of the code into the E ring and, in
+// the fused plan, the layer-0 gate of column 1.  m: the CTA's sample (global clip index); q as in sample_draw.
+template <int MB, bool WARP = false>
+__device__ void run_sample_task(const PixTask& t, const PixArgs& A, int r, int m, float* red, const float (&q)[8]) {
+  constexpr int SEG = PIX_D * MB;
+  const int tid = threadIdx.x;
+  const int c = t.col;
+  const long long code = sample_draw<WARP>(A, CtaBar(), [&](int j) { return A.arena + A.lay.LOG + ax<MB>(tid + 256 * j, m); },
+                                           A.arena + A.lay.LOG + (m ^ 1), MB, m, r, c, red, q);
   // embedding gather into the ring slot of this row (x_v = x_h = embedding(code) at layer 0)
   A.arena[A.lay.E + ((r & 3) * 2 + c) * SEG + ax<MB>(tid, m)] = A.emb[(size_t)code * PIX_D + tid];
   if (t.K) {
@@ -1635,7 +1509,7 @@ __device__ void run_sample_task(const PixTask& t, const PixArgs& A, int r, int m
     const float2 tw = *reinterpret_cast<const float2*>(A.blob + t.wofs + (size_t)code * (2 * PIX_D) + 2 * tid);
     const float* v2h = A.arena + A.lay.V2H + ((0 * 2 + 1) * 2) * SEG;
     if constexpr (WARP) {
-      if (A.style) {   // position (r, 1): row r of the schedule
+      if (A.draw.style) {   // position (r, 1): row r of the schedule
         float ct, cs;
         style_pair(A.cls_w, style_row(A, m, r), A.ncls, PIX_D, tid, ct, cs);
         const float zt = (__ldcg(v2h + ax<MB>(tid, m)) + tw.x) + ct;
@@ -1665,7 +1539,7 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
 // has its weights, leaves the grid barrier, finishes its task and has arrived again (ts_pixelcnn_trace): the
 // measurement the stage cost model and the CTA split should be fitted to.  The default kernel is TRACE = false.
 // WARP: the sample stage applies the sampling controls of A (ts_pixelcnn_sample); every other stage is unchanged.
-template <bool PERSISTENT, int PIPE, bool TRACE = false, bool S2 = false, int MB = 64, bool WARP = false>
+template <bool PERSISTENT, bool TRACE = false, bool S2 = false, int MB = 64, bool WARP = false>
 __global__ void __launch_bounds__(PIX_THREADS, 1) pixelcnn_kernel(PixArgs A, int r_single, int s_single) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float* wbuf = reinterpret_cast<float*>(smem_raw);
@@ -1680,13 +1554,16 @@ __global__ void __launch_bounds__(PIX_THREADS, 1) pixelcnn_kernel(PixArgs A, int
     if (!task_active(t, r_single, A.log_r0)) return;
     if (t.epi == EPI_SAMPLE) {
       if (cta < A.B) {
+        float q[8];
+        if (r_single >= A.T0 && (!WARP || draw_temperature(A, draw_index(A, cta)) > 0.f))
+          draw_noise<WARP>(A, r_single, t.col, cta, q);   // greedy: no noise
         if constexpr (WARP) {   // the shaping inputs of the draw (ts_pixelcnn_sample_shaped)
-          if (r_single >= A.T0 && (A.clip_shape || A.code_bias)) {
+          if (r_single >= A.T0 && (A.draw.clip_shape || A.draw.code_bias)) {
             shape_stage(A, cta, r_single, t.col, red, CtaBar());
             __syncthreads();
           }
         }
-        run_sample_task<MB, false, WARP>(t, A, r_single, cta, red);
+        run_sample_task<MB, WARP>(t, A, r_single, cta, red, q);
       }
       return;
     }
@@ -1694,7 +1571,7 @@ __global__ void __launch_bounds__(PIX_THREADS, 1) pixelcnn_kernel(PixArgs A, int
     for (int i = tid; i < nf; i += PIX_THREADS) wbuf[i] = A.blob[t.wofs + i];
     __syncthreads();
     EpiPre pre; pre.a = pre.b = 0.f; pre.valid = false;
-    run_matmul_task<0, MB, S2, WARP>(t, A, r_single, wbuf, red, pre);
+    run_matmul_task<MB, S2, WARP>(t, A, r_single, wbuf, red, pre);
     return;
   }
 
@@ -1741,9 +1618,9 @@ __global__ void __launch_bounds__(PIX_THREADS, 1) pixelcnn_kernel(PixArgs A, int
     // loaded / computed before the barrier wait, so it overlaps the wait
     float qpre[8];
     if (active && t.epi == EPI_SAMPLE && cta < A.B && r >= A.T0 && (!WARP || draw_temperature(A, draw_index(A, cta)) > 0.f))
-      draw_noise_of<WARP>(A, r, t.col, cta, qpre);   // greedy: no noise
+      draw_noise<WARP>(A, r, t.col, cta, qpre);   // greedy: no noise
     if constexpr (WARP) {   // the shaping inputs of this draw (ts_pixelcnn_sample_shaped), likewise before the wait
-      if (active && t.epi == EPI_SAMPLE && cta < A.B && r >= A.T0 && (A.clip_shape || A.code_bias))
+      if (active && t.epi == EPI_SAMPLE && cta < A.B && r >= A.T0 && (A.draw.clip_shape || A.draw.code_bias))
         shape_stage(A, cta, r, t.col, red, CtaBar());
     }
     if (has_w) { mbar_wait(&bars[buf], uses[buf] & 1u); uses[buf]++; }
@@ -1755,9 +1632,9 @@ __global__ void __launch_bounds__(PIX_THREADS, 1) pixelcnn_kernel(PixArgs A, int
     if constexpr (TRACE) { if (tr) tr[1] = globaltimer_ns(); }
     if (active) {
       if (t.epi == EPI_SAMPLE) {
-        if (cta < A.B) run_sample_task<MB, true, WARP>(t, A, r, cta, red, qpre);
+        if (cta < A.B) run_sample_task<MB, WARP>(t, A, r, cta, red, qpre);
       }
-      else run_matmul_task<PIPE, MB, S2, WARP>(t, A, r, wbuf + buf * PIX_WBUF, red, pre);
+      else run_matmul_task<MB, S2, WARP>(t, A, r, wbuf + buf * PIX_WBUF, red, pre);
     }
     if constexpr (TRACE) { __syncthreads(); if (tr) tr[2] = globaltimer_ns(); }
     grid_arrive(A.barrier);
@@ -1835,9 +1712,7 @@ __global__ void logits_to_ref_kernel(const float* __restrict__ in, float* __rest
 
 static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t* label, const float* noise, int noise_B,
                            int64_t* idx_out, float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s,
-                           bool logits_all, const SampleCtl* ctl, const int64_t* seeds, const int64_t* anchors,
-                           const float* style, const ts_clip_ctl* clip_ctl, const ts_clip_shape* clip_shape,
-                           const float* code_bias, const float* guide) {
+                           bool logits_all, const SampleCtl& d) {
   PixelPlan* P = e->pix;
   Plan3* Q = (Plan3*)P->p3;
   const int Ttot = T0 + T, D = P->D;
@@ -1864,8 +1739,7 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
   (void)noise_B;
 
   if (v3) {   // cluster-resident executor (pixelcnn3.inc): any batch size, clusters of 16 CTAs per 4 / 8 samples
-    launch_pixelcnn3(e, P, Q, audv, audh, label, noise, idx_out, logits_out, B, T0, Ttot, pre, logits_all, arena3, MB3, s, ctl, seeds,
-                     anchors, style, clip_ctl, clip_shape, code_bias, guide);
+    launch_pixelcnn3(e, P, Q, audv, audh, label, noise, idx_out, logits_out, B, T0, Ttot, pre, logits_all, arena3, MB3, s, d);
     return;
   }
   if (B > PIX_MB)
@@ -1893,30 +1767,21 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
   A.B = B; A.T0 = T0; A.Ttot = Ttot; A.log_r0 = logits_all ? 0 : T0; A.L = P->L; A.nstages = P->nstages; A.ncta = P->ncta;
   A.fused = P->fused ? 1 : 0;
   A.trace = P->d_trace; A.trace_row = P->trace_row;
-  const SampleCtl c = ctl ? *ctl : SampleCtl();
-  A.temperature = c.temperature; A.top_k = c.top_k; A.logp_out = c.logp_out;
-  A.top_p = c.top_p; A.min_p = c.min_p; A.kept_out = c.kept_out;
-  A.seeds = seeds;
-  A.anchors = anchors;
-  A.style = style; A.cls_w = P->d_cls; A.ncls = P->nclasses;
-  A.clip_ctl = clip_ctl;
-  A.clip_shape = clip_shape; A.code_bias = code_bias;
-  A.guide = guide;
+  A.draw = d;
+  A.cls_w = P->d_cls; A.ncls = P->nclasses;
   if (e->pixel_mode == 0) {
-    // A/B switch: 0 = burst loads + scalar FFMA, 4 = pipelined loads + scalar FFMA, 5 (default) = pipelined loads + paired FMAs (fma2)
-    static const int pipe = getenv("TS_PIX_PIPE") ? atoi(getenv("TS_PIX_PIPE")) : 5;
-    void* fn = pipe == 0 ? (void*)pixelcnn_kernel<true, 0> : pipe == 4 ? (void*)pixelcnn_kernel<true, 4> : (void*)pixelcnn_kernel<true, 5>;
-    if (MB == 32) fn = (void*)pixelcnn_kernel<true, 5, false, false, 32>;
-    if (MB == 16) fn = (void*)pixelcnn_kernel<true, 5, false, false, 16>;
-    if (MB == 8) fn = (void*)pixelcnn_kernel<true, 5, false, false, 8>;
-    if (tracing) fn = MB == 16 ? (void*)pixelcnn_kernel<true, 5, true, false, 16> : (void*)pixelcnn_kernel<true, 5, true>;
-    if (P->sched == 2) fn = tracing ? (void*)pixelcnn_kernel<true, 5, true, true> : (void*)pixelcnn_kernel<true, 5, false, true>;
-    if (ctl) {   // sampling controls: the WARP instantiation of the default pipeline (no stage-trace variant)
-      fn = MB == 8 ? (void*)pixelcnn_kernel<true, 5, false, false, 8, true>
-           : MB == 16 ? (void*)pixelcnn_kernel<true, 5, false, false, 16, true>
-           : MB == 32 ? (void*)pixelcnn_kernel<true, 5, false, false, 32, true>
-           : P->sched == 2 ? (void*)pixelcnn_kernel<true, 5, false, true, 64, true>
-                           : (void*)pixelcnn_kernel<true, 5, false, false, 64, true>;
+    void* fn = (void*)pixelcnn_kernel<true>;
+    if (MB == 32) fn = (void*)pixelcnn_kernel<true, false, false, 32>;
+    if (MB == 16) fn = (void*)pixelcnn_kernel<true, false, false, 16>;
+    if (MB == 8) fn = (void*)pixelcnn_kernel<true, false, false, 8>;
+    if (tracing) fn = MB == 16 ? (void*)pixelcnn_kernel<true, true, false, 16> : (void*)pixelcnn_kernel<true, true>;
+    if (P->sched == 2) fn = tracing ? (void*)pixelcnn_kernel<true, true, true> : (void*)pixelcnn_kernel<true, false, true>;
+    if (d.warp()) {   // the WARP instantiation of the default pipeline (no stage-trace variant)
+      fn = MB == 8 ? (void*)pixelcnn_kernel<true, false, false, 8, true>
+           : MB == 16 ? (void*)pixelcnn_kernel<true, false, false, 16, true>
+           : MB == 32 ? (void*)pixelcnn_kernel<true, false, false, 32, true>
+           : P->sched == 2 ? (void*)pixelcnn_kernel<true, false, true, 64, true>
+                           : (void*)pixelcnn_kernel<true, false, false, 64, true>;
     }
     TS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PIX_SMEM));
     int rs = 0, ss = 0;
@@ -1944,16 +1809,16 @@ static void generate_chunk(ts_engine* e, const Act3& aud, int b0, const int64_t*
     if (P->timing) { TS_CUDA(cudaEventRecord(P->ev1, s)); P->timed_rows += Ttot; P->timed_launches++; P->pending = true; }
     e->launches++;
   } else {
-    void (*fn1)(PixArgs, int, int) = P->sched == 2 ? pixelcnn_kernel<false, 0, false, true> : pixelcnn_kernel<false, 0>;
-    if (MB == 32) fn1 = pixelcnn_kernel<false, 0, false, false, 32>;
-    if (MB == 16) fn1 = pixelcnn_kernel<false, 0, false, false, 16>;
-    if (MB == 8) fn1 = pixelcnn_kernel<false, 0, false, false, 8>;
-    if (ctl) {
-      fn1 = MB == 8 ? pixelcnn_kernel<false, 0, false, false, 8, true>
-            : MB == 16 ? pixelcnn_kernel<false, 0, false, false, 16, true>
-            : MB == 32 ? pixelcnn_kernel<false, 0, false, false, 32, true>
-            : P->sched == 2 ? pixelcnn_kernel<false, 0, false, true, 64, true>
-                            : pixelcnn_kernel<false, 0, false, false, 64, true>;
+    void (*fn1)(PixArgs, int, int) = P->sched == 2 ? pixelcnn_kernel<false, false, true> : pixelcnn_kernel<false>;
+    if (MB == 32) fn1 = pixelcnn_kernel<false, false, false, 32>;
+    if (MB == 16) fn1 = pixelcnn_kernel<false, false, false, 16>;
+    if (MB == 8) fn1 = pixelcnn_kernel<false, false, false, 8>;
+    if (d.warp()) {
+      fn1 = MB == 8 ? pixelcnn_kernel<false, false, false, 8, true>
+            : MB == 16 ? pixelcnn_kernel<false, false, false, 16, true>
+            : MB == 32 ? pixelcnn_kernel<false, false, false, 32, true>
+            : P->sched == 2 ? pixelcnn_kernel<false, false, true, 64, true>
+                            : pixelcnn_kernel<false, false, false, 64, true>;
     }
     TS_CUDA(cudaFuncSetAttribute(fn1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PIX_SMEM));
     for (int r = 0; r < Ttot; ++r)
@@ -1975,34 +1840,31 @@ void pixel_destroy(ts_engine* e) {
 
 void pixelcnn_generate_act(ts_engine* e, const Act3& aud, const int64_t* label, const float* noise, int64_t* idx_out,
                            float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s, bool logits_all,
-                           const SampleCtl* ctl, const int64_t* seeds, const int64_t* anchors, const float* style,
-                           const ts_clip_ctl* clip_ctl, const ts_clip_shape* clip_shape, const float* code_bias,
-                           const float* guide) {
+                           const SampleCtl& d) {
   if (!e->pix) fail(TS_ERR_NOT_LOADED, "pixelcnn weights not loaded");
-  // an anchored, styled, per-clip, shaped or guided call always runs the WARP kernels; without controls at temperature 1,
-  // top_k 0 (the default draw's bits)
-  const SampleCtl dflt;
-  if ((anchors || style || clip_ctl || clip_shape || code_bias || guide) && !ctl) ctl = &dflt;
+  // an anchored, styled, per-clip, shaped or guided call always runs the WARP kernels (d.warp()); without controls at
+  // temperature 1, top_k 0 (the default draw's bits)
   // per-clip (guided: per-pair) controls, shaping and scales: host entries (validated by the caller) -> workspace, in
   // stream order before the sampler reads them
-  const size_t nd = guide ? (size_t)B / 2 : (size_t)B;
-  ts_clip_ctl* dclip = clip_ctl ? e->ws.alloc<ts_clip_ctl>(nd) : nullptr;
+  SampleCtl dd = d;
+  const size_t nd = d.guide ? (size_t)B / 2 : (size_t)B;
+  ts_clip_ctl* dclip = d.clip_ctl ? e->ws.alloc<ts_clip_ctl>(nd) : nullptr;
   if (dclip && !e->ws.sizing)
-    TS_CUDA(cudaMemcpyAsync(dclip, clip_ctl, nd * sizeof(ts_clip_ctl), cudaMemcpyHostToDevice, s));
-  ts_clip_shape* dshape = clip_shape ? e->ws.alloc<ts_clip_shape>(nd) : nullptr;
+    TS_CUDA(cudaMemcpyAsync(dclip, d.clip_ctl, nd * sizeof(ts_clip_ctl), cudaMemcpyHostToDevice, s));
+  ts_clip_shape* dshape = d.clip_shape ? e->ws.alloc<ts_clip_shape>(nd) : nullptr;
   if (dshape && !e->ws.sizing)
-    TS_CUDA(cudaMemcpyAsync(dshape, clip_shape, nd * sizeof(ts_clip_shape), cudaMemcpyHostToDevice, s));
-  float* dguide = guide ? e->ws.alloc<float>(nd) : nullptr;
-  if (dguide && !e->ws.sizing) TS_CUDA(cudaMemcpyAsync(dguide, guide, nd * sizeof(float), cudaMemcpyHostToDevice, s));
+    TS_CUDA(cudaMemcpyAsync(dshape, d.clip_shape, nd * sizeof(ts_clip_shape), cudaMemcpyHostToDevice, s));
+  float* dguide = d.guide ? e->ws.alloc<float>(nd) : nullptr;
+  if (dguide && !e->ws.sizing) TS_CUDA(cudaMemcpyAsync(dguide, d.guide, nd * sizeof(float), cudaMemcpyHostToDevice, s));
+  dd.clip_ctl = dclip; dd.clip_shape = dshape; dd.guide = dguide;
   // guided: pre_latents [P][T0][2] -> one copy per branch [2P][T0][2], so every pre read stays on the branch's own index
-  int64_t* dpre = guide && pre && T0 > 0 ? e->ws.alloc<int64_t>((size_t)B * T0 * 2) : nullptr;
+  int64_t* dpre = d.guide && pre && T0 > 0 ? e->ws.alloc<int64_t>((size_t)B * T0 * 2) : nullptr;
   if (dpre && !e->ws.sizing) {
     const size_t row = (size_t)T0 * 2 * sizeof(int64_t);
     for (int k = 0; k < 2; ++k)
       TS_CUDA(cudaMemcpy2DAsync(reinterpret_cast<char*>(dpre) + k * row, 2 * row, pre, row, row, nd, cudaMemcpyDeviceToDevice, s));
   }
-  generate_chunk(e, aud, 0, label, noise, B, idx_out, logits_out, B, T, dpre ? dpre : pre, T0, s, logits_all, ctl, seeds,
-                 anchors, style, dclip, dshape, code_bias, dguide);
+  generate_chunk(e, aud, 0, label, noise, B, idx_out, logits_out, B, T, dpre ? dpre : pre, T0, s, logits_all, dd);
 }
 
 void check_style(const ts_engine* e, const int64_t* label, const float* style, int ncls, const char* who) {
@@ -2086,6 +1948,7 @@ SampleCtl sample_ctl_of(const ts_sample_ctl* c) {
   SampleCtl s;
   s.temperature = c->temperature; s.top_k = c->top_k; s.top_p = c->top_p; s.min_p = c->min_p;
   s.logp_out = c->logp_out; s.kept_out = c->kept_out;
+  s.controls = true;
   return s;
 }
 
@@ -2216,23 +2079,18 @@ static void check_pix(ts_engine* e, int B, int T) {
   if (B <= 0 || T <= 0) fail(TS_ERR_INVALID, "pixelcnn: B=%d T=%d", B, T);
 }
 
-// ctl = nullptr: the default sampler (ts_pixelcnn_generate); else the sampling controls of ts_pixelcnn_sample.
-// seeds (ts_pixelcnn_sample_seeded): the draws' noise comes from the per-clip seeds instead of `noise`.
+// d: the draw inputs (SampleCtl), the default sampler (ts_pixelcnn_generate) when they are the defaults.
 static void pixelcnn_generate_call(ts_engine* e, const float* aud, const int64_t* label, const float* noise, int64_t* idx_out,
                                    float* logits_out, int B, int T, const int64_t* pre_latents, int T0, void* stream,
-                                   const SampleCtl* ctl, const int64_t* seeds = nullptr, const int64_t* anchors = nullptr,
-                                   const float* style = nullptr, const ts_clip_ctl* clip_ctl = nullptr,
-                                   const ts_clip_shape* clip_shape = nullptr, const float* code_bias = nullptr,
-                                   const float* guide = nullptr) {
+                                   const SampleCtl& d = SampleCtl()) {
   check_pix(e, B, T);
   if (T0 < 0 || (T0 > 0 && !pre_latents)) fail(TS_ERR_INVALID, "pixelcnn: T0=%d without pre_latents", T0);
-  if (ctl && !clip_ctl) check_sample_ctl(*ctl, noise, seeds);
+  if (d.controls && !d.clip_ctl) check_sample_ctl(d, noise, d.seeds);
   cudaStream_t s = (cudaStream_t)stream;
   auto body = [&] {
     Act3 a = new_act(e, B, T0 + T, 256, 0, s);
     nct_to_act(e, aud, 256, a, s);
-    pixelcnn_generate_act(e, a, label, noise, idx_out, logits_out, B, T, pre_latents, T0, s, false, ctl, seeds, anchors, style,
-                          clip_ctl, clip_shape, code_bias, guide);
+    pixelcnn_generate_act(e, a, label, noise, idx_out, logits_out, B, T, pre_latents, T0, s, false, d);
   };
   e->ws.begin_sizing(); body();
   size_t need = e->ws.need;
@@ -2244,7 +2102,7 @@ extern "C" int ts_pixelcnn_generate(ts_engine* e, const float* aud, const int64_
                                     int64_t* idx_out, float* logits_out, int B, int T, const int64_t* pre_latents, int T0,
                                     void* stream) {
   TS_API_BEGIN(e)
-  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, nullptr);
+  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream);
   TS_API_END(e)
 }
 
@@ -2260,7 +2118,7 @@ extern "C" int ts_pixelcnn_sample_ctl(ts_engine* e, const float* aud, const int6
                                       const ts_sample_ctl* ctl, void* stream) {
   TS_API_BEGIN(e)
   const SampleCtl c = sample_ctl_of(ctl);
-  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, &c);
+  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, c);
   TS_API_END(e)
 }
 
@@ -2291,13 +2149,11 @@ extern "C" int ts_pixelcnn_sample_seeded(ts_engine* e, const float* aud, const i
                                          const ts_sample_ctl* ctl, void* stream) {
   TS_API_BEGIN(e)
   check_pix(e, B, T);
-  if (ctl) {
-    const SampleCtl c = sample_ctl_of(ctl);
-    pixelcnn_generate_call(e, aud, label, nullptr, idx_out, logits_out, B, T, pre_latents, T0, stream, &c, seeds);
-  } else {
-    if (!seeds) fail(TS_ERR_INVALID, "ts_pixelcnn_sample_seeded: seeds is NULL (only greedy decoding runs without)");
-    pixelcnn_generate_call(e, aud, label, nullptr, idx_out, logits_out, B, T, pre_latents, T0, stream, nullptr, seeds);
-  }
+  SampleCtl c;
+  if (ctl) c = sample_ctl_of(ctl);
+  else if (!seeds) fail(TS_ERR_INVALID, "ts_pixelcnn_sample_seeded: seeds is NULL (only greedy decoding runs without)");
+  c.seeds = seeds;
+  pixelcnn_generate_call(e, aud, label, nullptr, idx_out, logits_out, B, T, pre_latents, T0, stream, c);
   TS_API_END(e)
 }
 
@@ -2312,8 +2168,8 @@ extern "C" int ts_pixelcnn_sample_anchored(ts_engine* e, const float* aud, const
   SampleCtl c;
   if (ctl) c = sample_ctl_of(ctl);
   check_anchored_source(ctl ? &c : nullptr, noise, seeds, "ts_pixelcnn_sample_anchored");
-  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, ctl ? &c : nullptr, seeds,
-                         anchors);
+  c.seeds = seeds; c.anchors = anchors;
+  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, c);
   TS_API_END(e)
 }
 
@@ -2329,8 +2185,8 @@ extern "C" int ts_pixelcnn_sample_styled(ts_engine* e, const float* aud, const i
   SampleCtl c;
   if (ctl) c = sample_ctl_of(ctl);
   check_anchored_source(ctl ? &c : nullptr, noise, seeds, "ts_pixelcnn_sample_styled");
-  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, ctl ? &c : nullptr, seeds,
-                         anchors, style);
+  c.seeds = seeds; c.anchors = anchors; c.style = style;
+  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, c);
   TS_API_END(e)
 }
 
@@ -2349,8 +2205,8 @@ extern "C" int ts_pixelcnn_sample_clips(ts_engine* e, const float* aud, const in
   check_clip_ctl(clip_ctl, B, noise, seeds, "ts_pixelcnn_sample_clips");
   SampleCtl c;   // logp_out / kept_out of ctl; the draws' controls come from clip_ctl
   if (ctl) { c.logp_out = ctl->logp_out; c.kept_out = ctl->kept_out; }
-  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, &c, seeds, anchors, style,
-                         clip_ctl);
+  c.seeds = seeds; c.anchors = anchors; c.style = style; c.clip_ctl = clip_ctl;
+  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, c);
   TS_API_END(e)
 }
 
@@ -2369,9 +2225,9 @@ extern "C" int ts_pixelcnn_sample_shaped(ts_engine* e, const float* aud, const i
   check_pix(e, B, T);
   check_style(e, label, style, ncls, "ts_pixelcnn_sample_shaped");
   if (clip_shape) check_clip_shape(clip_shape, B, "ts_pixelcnn_sample_shaped");
-  const SampleCtl c = shaped_ctl(ctl, clip_ctl, B, noise, seeds, "ts_pixelcnn_sample_shaped");
-  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, &c, seeds, anchors, style,
-                         clip_ctl, clip_shape, code_bias);
+  SampleCtl c = shaped_ctl(ctl, clip_ctl, B, noise, seeds, "ts_pixelcnn_sample_shaped");
+  c.seeds = seeds; c.anchors = anchors; c.style = style; c.clip_ctl = clip_ctl; c.clip_shape = clip_shape; c.code_bias = code_bias;
+  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, B, T, pre_latents, T0, stream, c);
   TS_API_END(e)
 }
 
@@ -2388,9 +2244,10 @@ extern "C" int ts_pixelcnn_sample_guided(ts_engine* e, const float* aud, const i
   check_style(e, label, style, ncls, "ts_pixelcnn_sample_guided");
   check_guidance(guidance, P, "ts_pixelcnn_sample_guided");
   if (clip_shape) check_clip_shape(clip_shape, P, "ts_pixelcnn_sample_guided");
-  const SampleCtl c = shaped_ctl(ctl, clip_ctl, P, noise, seeds, "ts_pixelcnn_sample_guided");
-  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, 2 * P, T, pre_latents, T0, stream, &c, seeds, anchors,
-                         style, clip_ctl, clip_shape, code_bias, guidance);
+  SampleCtl c = shaped_ctl(ctl, clip_ctl, P, noise, seeds, "ts_pixelcnn_sample_guided");
+  c.seeds = seeds; c.anchors = anchors; c.style = style; c.clip_ctl = clip_ctl; c.clip_shape = clip_shape; c.code_bias = code_bias;
+  c.guide = guidance;
+  pixelcnn_generate_call(e, aud, label, noise, idx_out, logits_out, 2 * P, T, pre_latents, T0, stream, c);
   TS_API_END(e)
 }
 

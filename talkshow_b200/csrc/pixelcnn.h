@@ -71,8 +71,12 @@ struct PixelPlan {
   int64_t timed_rows = 0, timed_launches = 0;
 };
 
-// Sampling controls of ts_pixelcnn_sample_ctl / ts_body_sample_ctl (include/talkshow_b200.h).  A call without them runs the
-// default sampler kernels; a call with them runs the WARP instantiations, whose only difference is the draw.
+// The draw inputs of one sampler call (include/talkshow_b200.h): the sampling controls of ts_pixelcnn_sample_ctl and the
+// inputs of the seeded, anchored, styled, per-clip, shaped and guided calls.  The C entry points fill it from their
+// arguments; the sampler kernels take it as the last member of their arguments (the fields the default kernels read keep
+// their offsets).  A call without controls or any of the WARP inputs runs the default sampler kernels; any other call runs
+// the WARP instantiations, whose only difference is the draw.  clip_ctl, clip_shape and guide are host memory up to
+// pixelcnn_generate_act, which copies them to the workspace; the kernels read device copies.
 struct SampleCtl {
   float temperature = 1.f;   // > 0: softmax(l / temperature); 0: greedy (first-index argmax of l, noise unread)
   int top_k = 0;             // 0 or 2048: off; else keep codes with l >= the k-th largest logit
@@ -80,6 +84,17 @@ struct SampleCtl {
   float top_p = 1.f;         // < 1: nucleus sampling on integer masses (nucleus_key, pixelcnn.cu); 1: off
   float min_p = 0.f;         // > 0: keep codes with exp(l / t - max l / t) >= min_p; 0: off
   int* kept_out = nullptr;   // [B,T,2] size of each draw's final keep set, or null
+  const int64_t* seeds = nullptr;           // [B] (device) per-clip seeds (ts_pixelcnn_sample_seeded); noise is then unread
+  const int64_t* anchors = nullptr;         // [B,T,2] (device) pinned draws (ts_pixelcnn_sample_anchored)
+  const float* style = nullptr;             // [B,T0+T,ncls] (device) speaker schedule (ts_pixelcnn_sample_styled), label unread
+  const ts_clip_ctl* clip_ctl = nullptr;    // [B] per-clip controls in place of the four above (ts_pixelcnn_sample_clips)
+  const ts_clip_shape* clip_shape = nullptr;  // [B] repetition penalty and window (ts_pixelcnn_sample_shaped)
+  const float* code_bias = nullptr;         // [B,2,2048] (device) code bias (ts_pixelcnn_sample_shaped)
+  const float* guide = nullptr;             // [B / 2] guidance scale per pair (ts_pixelcnn_sample_guided)
+  bool controls = false;                    // the call gave sampling controls (sample_ctl_of)
+  bool warp() const {
+    return controls || anchors || style || clip_ctl || clip_shape || code_bias || guide;
+  }
 };
 // Validates the controls (TS_ERR_INVALID): temperature finite and >= 0, top_k in [0, 2048], top_p in (0, 1], min_p in
 // [0, 1], noise (or seeds) given when sampling.
@@ -87,23 +102,14 @@ void check_sample_ctl(const SampleCtl& c, const float* noise, const int64_t* see
 // The public struct as the internal one (TS_ERR_INVALID when null).
 SampleCtl sample_ctl_of(const ts_sample_ctl* c);
 
-// aud: AudioEncoder output, channel-last [B, T0+T, 256].  ctl = nullptr: the default sampler.  seeds [B] (device): the
-// draws' noise is computed from the per-clip seeds (ts_pixelcnn_sample_seeded) and `noise` is not read.  anchors
-// [B,T,2] (device): the pinned draws of ts_pixelcnn_sample_anchored; the call then runs the WARP kernels, at the default
-// controls when ctl is null.  style [B,T0+T,ncls] (device): the speaker schedule of ts_pixelcnn_sample_styled (label
-// unread), likewise on the WARP kernels.  clip_ctl [B] (HOST, validated with check_clip_ctl): the per-clip controls of
-// ts_pixelcnn_sample_clips, copied to the workspace on s; each clip draws with its entry in place of ctl's four controls.
-// clip_shape [B] (HOST, validated with check_clip_shape) and code_bias [B,2,2048] (device): the logit shaping of
-// ts_pixelcnn_sample_shaped, likewise on the WARP kernels (clip_shape copied to the workspace on s).
-// guide [B / 2] (HOST, validated with check_guidance): the scales of ts_pixelcnn_sample_guided, copied to the workspace on
-// s.  B is then the branch count 2P: aud, label, style, idx_out and logits_out are per branch; noise [2T][P][2048], seeds,
-// anchors, pre, clip_ctl, clip_shape and code_bias are per pair (pre is copied once per branch into the workspace).
+// aud: AudioEncoder output, channel-last [B, T0+T, 256].  d: the draw inputs (SampleCtl; the default draw when
+// d.warp() is false).  clip_ctl, clip_shape (validated with check_clip_ctl / check_clip_shape) and guide (validated with
+// check_guidance) are read from host memory and copied to the workspace on s.  Guided: B is the branch count 2P; aud,
+// label, style, idx_out and logits_out are per branch; noise [2T][P][2048], seeds, anchors, pre, clip_ctl, clip_shape and
+// code_bias are per pair (pre is copied once per branch into the workspace).
 void pixelcnn_generate_act(ts_engine* e, const Act3& aud, const int64_t* label, const float* noise, int64_t* idx_out,
                            float* logits_out, int B, int T, const int64_t* pre, int T0, cudaStream_t s,
-                           bool logits_all = false, const SampleCtl* ctl = nullptr, const int64_t* seeds = nullptr,
-                           const int64_t* anchors = nullptr, const float* style = nullptr,
-                           const ts_clip_ctl* clip_ctl = nullptr, const ts_clip_shape* clip_shape = nullptr,
-                           const float* code_bias = nullptr, const float* guide = nullptr);
+                           bool logits_all = false, const SampleCtl& d = SampleCtl());
 // The class terms of gate channel q (tanh half) and D + q (sigmoid half) under one row's speaker weights w[0..ncls)
 // (ts_pixelcnn_sample_styled): acc = w0 E[0][ch], then acc + w_s E[s][ch] for s = 1 .. ncls-1, every product and sum
 // rounded to fp32 without contraction.  tab: one layer's class_cond_embedding [ncls][2D]; w null (a padding sample of the
